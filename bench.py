@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Headline benchmark: GPT-2 345M training throughput (tokens/s, whole job) on N B200s of one node.
+"""Headline benchmark: GPT-2 345M training throughput (tokens/s, whole job) on N H100s of one node.
 
-Contract (driver): `python bench.py --gpus N --steps K --warmup W` (N>1 via torch.distributed.run), one JSON
-line from rank 0.  Metric/config = BASELINE.json: GPT-2 (examples/GPT2/345M.json: 24 layers, d=1024,
+`python bench.py --gpus N --steps K --warmup W` (N>1 via torch.distributed.run) prints one JSON line from rank 0.
+`--dump-outputs DIR` additionally writes what the last timed step computed (see dump_outputs) so that two builds can be
+compared output for output: inputs and initial weights are seeded, identical from run to run.  Metric/config = BASELINE.json: GPT-2 (examples/GPT2/345M.json: 24 layers, d=1024,
 16 heads, ctx 1024, vocab 50257, batch 4 per model replica, AdamW), bf16 compute / fp32 master+optimizer,
 synthetic `fake_input` tokens, random-init weights.  Every step = forward + backward + gradient sync +
 optimizer update.  `--impl reference` is the reference arm (see DESIGN.md: the TensorFlow-fork reference
@@ -50,6 +51,23 @@ def summarize_clocks(samples):
             "samples": len(samples)}
 
 
+DUMP_SAMPLE = 1 << 22   # parameter elements written by --dump-outputs (16 MB of float32)
+
+
+def dump_outputs(out_dir, loss, params):
+    """What a caller of the timed step receives after the last timed step: the loss, and the bf16 compute parameters the
+    optimizer update produced -- the copy every rank holds in full under data parallelism (the fused sharded optimizer
+    all-gathers it) -- as a fixed-stride sample of the flat buffer when it has more than DUMP_SAMPLE elements."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(-1).cpu().numpy())
+    if params is not None:
+        flat = params.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            flat = flat[::flat.numel() // DUMP_SAMPLE][:DUMP_SAMPLE]
+        np.save(os.path.join(out_dir, "params_sample.npy"), flat.float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -65,6 +83,9 @@ def main():
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-exposed", action="store_true", help="skip the exposed-communication measurement (N > 1)")
     ap.add_argument("--no-tp", action="store_true", help="skip the tensor-parallel arm (N > 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss and a fixed sample of the updated bf16 parameters as DIR/*.npy "
+                         "(loss only for --impl library)")
     ap.add_argument("--no-library-arm", action="store_true",
                     help="skip the same-box library comparator (cuBLAS / SDPA / per-tensor NCCL step, bench/torch_baseline.py)")
     args = ap.parse_args()
@@ -72,7 +93,7 @@ def main():
     if args.impl == "reference":
         print(json.dumps({"impl": "reference", "unavailable":
                           "alibaba/TePDist is a Bazel-2.0 fork of mid-2020 TensorFlow (no setup.py/pyproject; CUDA 10/11, sm<=80); "
-                          "pip install --no-index of /root/reference fails: not installable offline"}))
+                          "it cannot be installed offline"}))
         return 0
 
     if os.environ.get("TEPDIST_HANG_DUMP"):
@@ -159,6 +180,8 @@ def main():
     ms = e0.elapsed_time(e1)
     launches = ops.launch_count()
     final_loss = float(loss)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, None if library else trainer.executor().store.compute)
 
     # ---------------- end-to-end through the public API: H2D inputs from pinned memory + D2H loss every step
     barrier()
@@ -290,7 +313,7 @@ def main():
                        "global_batch": B * world, "per_gpu_batch": B, "seq_len": S, "vocab": cfg.n_vocab,
                        "optimizer": "AdamW (fp32 master + moments)", "parallelism": parallelism if library else trainer.plan_info.get("parallelism", f"dp{world}"),
                        "cuda_graph": (lt.use_graph if library else not args.no_graph), "comm": "nccl-per-tensor" if library else args.comm,
-                       "l2": "working set per step >> 126 MB L2 (0.7 GB bf16 weights + 5.7 GB fp32 optimizer state touched every step)"},
+                       "l2": "working set per step >> 50 MB L2 (0.7 GB bf16 weights + 5.7 GB fp32 optimizer state touched every step)"},
             "e2e": {"value": e2e, "unit": "tokens/s", "ms_per_step": ms_e2e / K,
                     "h2d_bytes_per_step": 2 * rows * S * 4 * world, "d2h_bytes_per_step": 4 * world},
             "gpu_launches": launches,

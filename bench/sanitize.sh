@@ -12,7 +12,7 @@
 #               global-memory flag protocols (symm_barrier, stream-K partial-tile flags, p2p_gather_chunks flags).
 #   synccheck : named-barrier / __syncwarp misuse (bar.sync 1,128 in the epilogues, softmax max exchange).
 #   initcheck : reads of never-written global memory (stream-K workspace, dQ accumulator, slot buffers).
-# Unknown until run: how much of the async proxy (TMA loads, tcgen05.mma operand reads, TMEM) the sanitizer models on sm_100a.
+# Unknown until run: how much of the async proxy (TMA loads, wgmma operand reads) the sanitizer models on sm_90a.
 # `gemm2` is left out by default: its check interleaves numerics with long timing loops.
 set -u
 tool="${1:-memcheck}"

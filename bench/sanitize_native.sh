@@ -3,7 +3,7 @@
 # their own compute-sanitizer script, bench/sanitize.sh).  Usage: bash bench/sanitize_native.sh [outdir]
 set -u
 root=$(cd "$(dirname "$0")/.." && pwd)
-out=${1:-$root/profiles/sanitizer_native}
+out=${1:-$root/sanitizer_logs}
 mkdir -p "$out"
 tmp=$(mktemp -d)
 src="$root/tests/native/data_loader_stress.cc $root/tepdist_b200/csrc/runtime/data_loader.cc"

@@ -22,8 +22,7 @@ def main():
     ap.add_argument("--optimizer", default="adamw", choices=["adamw", "adam", "momentum", "sgd"],
                     help="reference: AdamOptimizer(0.1) in train_imagenet.py, MomentumOptimizer(0.01, 0.9) in resnet_train.py")
     ap.add_argument("--lr", type=float, default=None)
-    ap.add_argument("--no-graph", action="store_true", help="run the step eagerly (default: whole step replayed from a CUDA graph: "
-                    "747 vs 480 examples/s on 2 x B200, 500M model, batch 4 per GPU)")
+    ap.add_argument("--no-graph", action="store_true", help="run the step eagerly (default: whole step replayed from a CUDA graph)")
     ap.add_argument("--graph", action="store_true", help="(default; kept for compatibility)")
     a = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))

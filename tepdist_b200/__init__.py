@@ -1,7 +1,7 @@
-"""tepdist_b200 — a B200-native automatic distributed-training system with TePDist's capabilities.
+"""tepdist_b200 — a H100-native automatic distributed-training system with TePDist's capabilities.
 
 Layers (see DESIGN.md): PyTorch client frontend -> planner IR -> C++ planner (SPMD cones/ILP, pipeline
-stage ILP, sync-free micro-batching) -> transforms -> task-graph runtime -> sm_100a kernels + NCCL /
+stage ILP, sync-free micro-batching) -> transforms -> task-graph runtime -> sm_90a kernels + NCCL /
 peer-memory collectives.
 """
 __version__ = "0.1.0"

@@ -1,8 +1,8 @@
-"""In-tree native build: sm_100a CUDA kernels (nvcc -> ops/libtepdist_kernels.so, C ABI loaded with
+"""In-tree native build: sm_90a CUDA kernels (nvcc -> ops/libtepdist_kernels.so, C ABI loaded with
 ctypes) and the C++ planner/runtime core (g++ + pybind11 -> tepdist_b200/_C*.so).
 
-Artifacts are built next to the sources so they travel with `gpurun` snapshots; nothing is JIT-cached
-outside the repository.  `python -m tepdist_b200.build_native [--force]`.
+Artifacts are built next to the sources (git-ignored), so the package imports from the source tree; nothing is
+JIT-cached outside the repository.  `python -m tepdist_b200.build_native [--force]`.
 """
 from __future__ import annotations
 
@@ -19,7 +19,7 @@ KERNEL_SO = os.path.join(ROOT, "ops", "libtepdist_kernels.so")
 CORE_SRC = os.path.join(ROOT, "csrc")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v",
 ]
 

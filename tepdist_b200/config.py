@@ -90,13 +90,13 @@ def schedule_overrides() -> Dict[str, Any]:
 
 
 def hw_profile():
-    """HW_PROFILE: cost-model constants of the planner / evaluator -- "b200" (default) or "reference_v100" (the reference's
+    """HW_PROFILE: cost-model constants of the planner / evaluator -- "h100" (default) or "reference_v100" (the reference's
     15 TFLOP/s / 300 GB/s constants, evaluator.h:47-56)."""
     from . import _C
-    name = env().get("HW_PROFILE") if is_set("HW_PROFILE") else "b200"
-    if name not in ("b200", "reference_v100"):
-        raise ValueError(f"HW_PROFILE={name!r}: expected 'b200' or 'reference_v100'")
-    return _C.HwProfile.reference_v100() if name == "reference_v100" else _C.HwProfile.b200()
+    name = env().get("HW_PROFILE") if is_set("HW_PROFILE") else "h100"
+    if name not in ("h100", "reference_v100"):
+        raise ValueError(f"HW_PROFILE={name!r}: expected 'h100' or 'reference_v100'")
+    return _C.HwProfile.reference_v100() if name == "reference_v100" else _C.HwProfile.h100()
 
 
 def pp_bandwidth() -> Optional[float]:
@@ -140,7 +140,7 @@ def comm_mode(requested: Optional[str]) -> str:
 
 
 def comm_dtype():
-    """FP16_COMM: fp32 sum-reductions travel in 16 bit (bf16 on B200; custom_collective_expander.cc FP16 wrap)."""
+    """FP16_COMM: fp32 sum-reductions travel in 16 bit (bf16 here; custom_collective_expander.cc FP16 wrap)."""
     import torch
     return torch.bfloat16 if is_set("FP16_COMM") and env().get_bool("FP16_COMM") else None
 

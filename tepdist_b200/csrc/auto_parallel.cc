@@ -398,7 +398,7 @@ ParallelPlan AutoParallelRun(const Graph& g, const AutoParallelOptions& opt) {
       ei.stage_flops = {fl};
       for (auto& n : cur.nodes) n.stage = 0;
     }
-    // gradient collectives overlap with backward on B200 (side stream); activation collectives are exposed
+    // gradient collectives overlap with backward (side stream); activation collectives are exposed
     ei.spmd_comm_bytes = spmd_comm * p.micro;
     ei.exposed_comm_fraction = opt.exposed_comm_fraction >= 0 ? opt.exposed_comm_fraction : opt.hw.ExposedCommFraction(p.spmd);
     ei.var_bytes = VarBytes(g);

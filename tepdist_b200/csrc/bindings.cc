@@ -166,7 +166,7 @@ PYBIND11_MODULE(_C, m) {
 
   py::class_<HwProfile>(m, "HwProfile")
       .def(py::init<>())
-      .def_static("b200", &HwProfile::B200)
+      .def_static("h100", &HwProfile::H100)
       .def_static("reference_v100", &HwProfile::ReferenceV100)
       .def_readwrite("name", &HwProfile::name)
       .def_readwrite("flops", &HwProfile::flops)
@@ -177,7 +177,8 @@ PYBIND11_MODULE(_C, m) {
       .def_readwrite("small_batch_half_rows", &HwProfile::small_batch_half_rows)
       .def("exposed_comm_fraction", &HwProfile::ExposedCommFraction)
       .def("compute_slowdown", &HwProfile::ComputeSlowdown)
-      .def_readwrite("mem_bytes", &HwProfile::mem_bytes);
+      .def_readwrite("mem_bytes", &HwProfile::mem_bytes)
+      .def_readwrite("var_mem_limit", &HwProfile::var_mem_limit);
 
   py::class_<SpmdOptions>(m, "SpmdOptions")
       .def(py::init<>())

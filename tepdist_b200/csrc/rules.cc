@@ -93,8 +93,7 @@ void LinearRule(Ctx& c, const RuleOptions& opt) {
   // y_partial = x_s w_s ; y[shard d] = reduce_scatter(y_partial) + b + res[shard d].  The residual stays split -- with the plain
   // "contract" candidate a fused residual has to be replicated, which prices a split residual stream as an all-gather per
   // layer that the rewritten graph never executes.  Cost: the reduce-scatter's bytes (the launch is added by the planner).
-  // Opt-in (SpmdOptions::sequence_parallel, strategy "tpsp"): the all-reduce form is what the fused NVLS chains execute and what
-  // the tensor-parallel numbers in profiles/ were measured on.
+  // Opt-in (SpmdOptions::sequence_parallel, strategy "tpsp"): the all-reduce form is what the fused NVLS chains execute.
   for (int d = 0; d < rx - 1 && opt.sequence_parallel; ++d)
     if (c.divisible(c.o(), d))
       c.add(mk(c.S(rx - 1), c.S(1), c.G(), c.S(d)), {c.S(d)}, "contract_rs" + std::to_string(d),

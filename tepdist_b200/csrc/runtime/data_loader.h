@@ -4,7 +4,7 @@
 // Reference parity (SURVEY K13 / F: examples/GPT2/inputs.py): the reference's client reads BPE token records through a
 // tf.data pipeline -- windows of n_ctx + 1 tokens cut into (input, next-token label), several datasets mixed by weight
 // (sample_from_datasets), prefetch a few batches, and a `fake_input` mode of random tokens.  Here the same capabilities without
-// a framework dependency, designed around what the training step needs on a B200 box: batches land directly in page-locked memory
+// a framework dependency, designed around what the training step needs on a GPU box: batches land directly in page-locked memory
 // that the step copies from asynchronously, and sampling is STATELESS -- sample k of the run is a pure function of (seed, k) --
 // so every data-parallel rank computes exactly its own rows of every global batch without coordination, and a resumed job
 // continues the stream from its step counter alone.

@@ -56,7 +56,7 @@ struct PipelineSpec {
   std::vector<double> act_bytes;                 // activation bytes stashed per (stage, micro) between fwd and bwd
   std::vector<double> boundary_bytes;            // bytes crossing boundary s -> s+1 per micro-batch (one direction)
   double p2p_bw = 7.7e11, p2p_latency = 5e-6;
-  double mem_limit = 180e9 * 0.9;
+  double mem_limit = HwProfile().mem_bytes;
 };
 // D3 CompileTaskDAG + CrossDeviceCalibration: per (stage, micro) Input/Compute/Output bundles for fwd and bwd, GA per
 // micro, GAInit/AG per stage, Send/Recv on every stage boundary.

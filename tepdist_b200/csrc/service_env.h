@@ -15,10 +15,10 @@ namespace tepdist {
   X(IGNORE_ANNOTATION, "true", "ignore user sharding annotations in cost mode")                    \
   X(AUX_AFFINITY, "false", "force optimizer slots to share their variable's layout")               \
   X(COST_FACTOR, "1.0", "weight of all-to-all bytes in the planner objective")                     \
-  X(FP16_COMM, "false", "communicate fp32 reductions in 16-bit (bf16 on B200)")                    \
+  X(FP16_COMM, "false", "communicate fp32 reductions in 16-bit (bf16)")                    \
   X(NUM_GRADIENTS, "0", "expected number of gradient tensors (sanity check)")                      \
   X(FORWARD_SUB_GRAPH_NUM, "0", "number of forward sub-graphs for the sub-graph DP (0 = every separator)") \
-  X(VAR_MEM_LIMIT, "150000000000", "bytes per device for variables+slots+grads before weights are force-sharded") \
+  X(VAR_MEM_LIMIT, "60000000000", "bytes per device for variables+slots+grads before weights are force-sharded") \
   X(OPT_LEVEL, "2", ">=3 whole-graph problem; <3 sub-graph DP; <1 fast inference only")            \
   X(UNBALANCED_RATIO, "0.08", "per-stage FLOPs slack of the pipeline planner")                     \
   X(NUM_MICRO_BATCHES, "0", "config mode: micro-batches")                                          \
@@ -37,8 +37,8 @@ namespace tepdist {
   X(DISABLE_BUFFER_ALIAS, "false", "debug: do not alias variable inputs/outputs")                  \
   X(FRONTEND, "torch", "client frontend name")                                                     \
   X(DUMP_ARTIFACTS, "false", "write strategies/cone/comm/stage/task-graph dumps (reference DUMP_LLVM_PTX analogue)") \
-  X(COMM_MODE, "fused", "fused = peer-memory sm_100a kernels, nccl = reference-semantics baseline") \
-  X(HW_PROFILE, "b200", "cost-model constants: b200 | reference_v100")
+  X(COMM_MODE, "fused", "fused = peer-memory sm_90a kernels, nccl = reference-semantics baseline") \
+  X(HW_PROFILE, "h100", "cost-model constants: h100 | reference_v100")
 
 class ServiceEnv {
  public:

@@ -21,7 +21,7 @@ namespace tepdist {
 
 struct SpmdOptions {
   int num = 2;                       // devices at this mesh level
-  double var_mem_limit = 150e9;      // VAR_MEM_LIMIT (bytes per device for variables + slots + grads)
+  double var_mem_limit = HwProfile().var_mem_limit;   // VAR_MEM_LIMIT (bytes per device for variables + slots + grads)
   int num_threads = 1;               // ILP_NUM_THREADS: sub-graph problems solved concurrently (same plan, less wall time)
   bool share_relayout_cost = false;  // experimental: split a value's re-layout price over its consumers (see EdgeCost)
   bool sequence_parallel = false;    // tensor-parallel plans may use the reduce-scatter / all-gather (Megatron sequence-parallel) form

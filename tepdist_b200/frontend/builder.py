@@ -57,7 +57,7 @@ class GraphBuilder:
     def constant(self, value: float, shape: Sequence[int] = (), dtype: str = "f32") -> Value:
         return self._n("constant", [], [TensorType(tuple(shape), dtype)], {"value": value}).out()
 
-    # ------------------------------------------------------------------ macro ops (map 1:1 onto sm_100a kernels)
+    # ------------------------------------------------------------------ macro ops (map 1:1 onto sm_90a kernels)
     def embedding(self, tokens: Value, wte: Value, wpe: Value, name="embed") -> Value:
         B, S = self.t(tokens).shape
         C = self.t(wte).shape[1]

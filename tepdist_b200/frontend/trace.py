@@ -189,7 +189,7 @@ def trace(module: nn.Module, example_inputs: Dict[str, torch.Tensor], loss: str 
             elif t in ("contiguous", "float", "to"):
                 env[node.name] = a[0]
             elif t is F.scaled_dot_product_attention:
-                # q, k, v: [B, H, S, D] -> the fused attention op (one tcgen05 flash-attention kernel on the GPU) on the
+                # q, k, v: [B, H, S, D] -> the fused attention op (one wgmma flash-attention kernel on the GPU) on the
                 # heads-major packed layout [B, S, H, 3, D]
                 if node.kwargs.get("attn_mask") is not None or node.kwargs.get("dropout_p", 0.0):
                     raise NotImplementedError("scaled_dot_product_attention: attn_mask / dropout are not supported")

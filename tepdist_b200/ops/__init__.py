@@ -1,4 +1,4 @@
-"""Device-op layer: hand-written sm_100a kernels behind a C ABI (``libtepdist_kernels.so``), loaded with
+"""Device-op layer: hand-written sm_90a kernels behind a C ABI (``libtepdist_kernels.so``), loaded with
 ctypes.  On CUDA tensors every op here runs OUR kernel and raises if the library is missing (no silent
 eager fallback); CPU tensors take a plain-PyTorch reference path that the tests also use as the oracle.
 
@@ -30,7 +30,7 @@ def lib() -> ctypes.CDLL:
     if _lib is None:
         if not os.path.exists(_LIB_PATH):
             raise KernelLibraryMissing(
-                f"{_LIB_PATH} not built; run `python -m tepdist_b200.build_native` (nvcc, sm_100a)")
+                f"{_LIB_PATH} not built; run `python -m tepdist_b200.build_native` (nvcc, sm_90a)")
         _lib = ctypes.CDLL(_LIB_PATH)
         for name in dir(_Sig):
             if name.startswith("tepd_"):
@@ -77,7 +77,6 @@ _vp, _i, _ll, _f = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_fl
 class _Sig:
     tepd_gemm_bf16 = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _ll, _ll, _ll, _ll, _ll, _ll, _ll,
                       _i, _i, _i, _i, _i, _i, _f, _i, _i, _i, _vp, _vp, _vp]
-    tepd_gemm2_bf16 = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _ll, _ll, _ll, _ll, _i, _i, _i, _f, _i, _vp, _i, _i, _i]
     tepd_layernorm_fwd = [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp]
     tepd_layernorm_bwd = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]
     tepd_gelu_fwd = [_vp, _vp, _ll, _vp]
@@ -166,7 +165,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     odd = a.is_cuda and (N % 8 != 0 or (a_mn and M % 8 != 0) or (K % 8 != 0 and not (a_mn and b_mn))
                          or a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16)
     if odd:
-        _warn_once(f"gemm {M}x{N}x{K} ({a.dtype}): shape / dtype outside the TMA alignment rules of the tcgen05 kernels, "
+        _warn_once(f"gemm {M}x{N}x{K} ({a.dtype}): shape / dtype outside the TMA alignment rules of the wgmma kernels, "
                    "running this one through torch.matmul")
     if not a.is_cuda or odd:  # reference path (CPU tests / oracle; odd shapes on the GPU)
         A = a3.float().transpose(1, 2) if a_mn else a3.float()
@@ -202,16 +201,6 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
         waves = -(-tiles // _sms())
         if tiles / (waves * _sms()) < 0.93:
             split_k = -1
-    if (USE_GEMM2 and not batched and not a_mn and not accumulate and out.dtype == torch.bfloat16 and M >= 256 and N >= 256
-            and block_n == 0 and split_k in (0, 1)):
-        res2 = None if residual is None else residual.reshape(M, N)
-        gemm2(a, b, b_mn=b_mn, bias=bias, residual=res2, act=act, out=out, out2=out2,
-              aux=None if aux is None else aux.reshape(M, N), alpha=alpha)
-        return out
-    if (USE_GEMM2 and not batched and a_mn and b_mn and not accumulate and out.dtype == torch.float32 and M >= 256 and N >= 256
-            and block_n == 0 and split_k in (0, 1) and bias is None and residual is None and act is None):
-        gemm2(a, b, a_mn=True, b_mn=True, out=out, alpha=alpha)     # weight gradient with plain stores
-        return out
     if bias is not None:
         assert bias.dtype in (torch.float32, torch.bfloat16) and bias.is_contiguous()
     res3 = None
@@ -224,8 +213,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
             tiles = ((M + 127) // 128) * ((N + 255) // 256) * batch
             kb = (K + 63) // 64
             if STREAM_K and tiles >= _sms():
-                split_k = -1    # stream-K: every SM gets the same number of k-blocks (fp32 red.add flush per tile); measured
-                                # neutral-to-better from one full wave of tiles up, worse than plain split-K below that
+                split_k = -1    # stream-K: every SM gets the same number of k-blocks (fp32 red.add flush per tile) once there
+                                # is at least one full wave of tiles; below that plain split-K
             else:
                 while tiles * split_k * 2 <= _sms() and split_k * 2 <= max(1, kb // 4):
                     split_k *= 2
@@ -245,32 +234,31 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
 
 STREAM_K_FWD = os.environ.get("TEPDIST_STREAM_K_FWD", "0") == "1"   # stream-K + fix-up for bf16-output GEMMs (opt-in)
 STREAM_K = os.environ.get("TEPDIST_STREAM_K", "1") == "1"  # stream-K scheduling for fp32-accumulate GEMMs (weight gradients)
-USE_GEMM2 = os.environ.get("TEPDIST_GEMM2", "1") == "1"   # 2-CTA (cta_group::2) kernel for eligible shapes (measured +1.7 % on the GPT-2 step)
 
 
 def wgrad_prefers_store(n_out: int, k_in: int) -> bool:
-    """Weight gradient [n_out, k_in]: plain-store 2-CTA GEMM when the 256x256 tiles fill at least half of the CTA pairs;
-    smaller outputs are better off split over K with fp32 red.add into a zero-filled slot (1-CTA kernel)."""
-    tiles = ((n_out + 255) // 256) * ((k_in + 255) // 256)
-    return USE_GEMM2 and n_out >= 256 and k_in >= 256 and n_out % 8 == 0 and k_in % 8 == 0 and tiles * 2 >= _sms() // 2
+    """Weight gradient [n_out, k_in]: plain-store GEMM when its 128x256 tiles fill at least half of the SMs; smaller outputs
+    are better off split over K with fp32 red.add into a zero-filled slot."""
+    tiles = ((n_out + 127) // 128) * ((k_in + 255) // 256)
+    return n_out >= 256 and k_in >= 256 and n_out % 8 == 0 and k_in % 8 == 0 and tiles >= _sms() // 2
 
 
 def _gemm2_stream_k(M: int, N: int, K: int, fp32_out: bool) -> bool:
-    """Measured (profiles/kernel_checks_trip22.json): the stream-K schedule of the 2-CTA kernel only pays for very large
-    plain-store outputs (lm_head weight gradient 50304x1024: 1466 vs 1245 TFLOP/s); on the 64..256-tile transformer shapes
-    the fix-up of split tiles (uncoalesced fp32 partial tiles through L2) costs more than the idle tail wave it removes."""
+    """Stream-K only for very large plain-store outputs (the lm_head weight gradient); on the transformer shapes the fix-up
+    of split tiles (fp32 partial tiles through L2) costs more than the idle tail wave it removes."""
     if not STREAM_K or not fp32_out:
         return False
-    tiles = ((M + 255) // 256) * ((N + 255) // 256)
-    return tiles >= 8 * (_sms() // 2)
+    tiles = ((M + 127) // 128) * ((N + 255) // 256)
+    return tiles >= 8 * _sms()
 
 
 def gemm2(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False, bias: Optional[torch.Tensor] = None,
           residual: Optional[torch.Tensor] = None, act: Optional[str] = None, out: Optional[torch.Tensor] = None,
           out2: Optional[torch.Tensor] = None, aux: Optional[torch.Tensor] = None, alpha: float = 1.0,
           out_dtype: torch.dtype = torch.bfloat16, stream_k: Optional[bool] = None) -> torch.Tensor:
-    """2-CTA tcgen05 GEMM (256x256 tile per CTA pair): a [M,K] (or [K,M] with a_mn), b [N,K] (or [K,N] with b_mn);
-    bf16 output with the fused epilogues or fp32 plain stores.  stream_k: None = decide from the wave occupancy."""
+    """Large-tile GEMM (128x256 output tile per CTA) with an explicit schedule choice: a [M,K] (or [K,M] with a_mn),
+    b [N,K] (or [K,N] with b_mn); bf16 output with the fused epilogues or fp32 plain stores.  stream_k: None = decide
+    from the output size, True = stream-K with fix-up of split tiles, False = one tile per CTA at a time."""
     M, K = (a.shape[1], a.shape[0]) if a_mn else a.shape
     N = b.shape[1] if b_mn else b.shape[0]
     if out is None:
@@ -279,18 +267,12 @@ def gemm2(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = 
     assert out.dtype in (torch.bfloat16, torch.float32)
     if stream_k is None:
         stream_k = _gemm2_stream_k(M, N, K, out.dtype == torch.float32)
-    rc = lib().tepd_gemm2_bf16(a.data_ptr(), b.data_ptr(), out.data_ptr(), _p(out2), _p(bias), _p(residual), _p(aux), M, N, K,
-                               a.stride(0), b.stride(0), out.stride(0), residual.stride(0) if residual is not None else 0,
-                               int(b_mn), {None: 0, "gelu": 1, "gelu_bwd": 2}[act],
-                               int(bias is not None and bias.dtype == torch.bfloat16), float(alpha), _sms(), _stream(),
-                               int(a_mn), int(out.dtype == torch.float32), int(bool(stream_k)))
-    _check(rc, "gemm2_bf16")
-    _count()
-    return out
+    return gemm(a, b, a_mn=a_mn, b_mn=b_mn, bias=bias, residual=residual, act=act, out=out, alpha=alpha,
+                split_k=-1 if stream_k else 1, block_n=256, out2=out2, aux=aux)
 
 
 def einsum(eq: str, a: torch.Tensor, b: torch.Tensor, _force: bool = False) -> torch.Tensor:
-    """Two-operand einsum as ONE batched tcgen05 GEMM (the expert FFNs / dispatch / combine of GPT-MoE and their gradients are
+    """Two-operand einsum as ONE batched wgmma GEMM (the expert FFNs / dispatch / combine of GPT-MoE and their gradients are
     einsums with a leading expert or group dim; the reference hands them to cuBLAS batched GEMMs, SURVEY 2.H K8).
 
     Indices are classified batch (in a, b, out) / M (a, out) / N (b, out) / K (a, b): each operand is brought to
@@ -421,7 +403,7 @@ CONV_NATIVE = os.environ.get("TEPDIST_CONV", "native") != "cudnn"   # "cudnn": l
 
 
 def conv_native_ok(x: torch.Tensor, w: torch.Tensor) -> bool:
-    """Own path: NHWC im2col / col2im kernels (conv_sm100.cu) around the tcgen05 GEMMs."""
+    """Own path: NHWC im2col / col2im kernels (conv_sm90.cu) around the wgmma GEMMs."""
     return CONV_NATIVE and x.is_cuda and x.dtype == torch.bfloat16 and w.shape[0] % 8 == 0
 
 
@@ -496,7 +478,7 @@ def conv2d_wgrad(dy: torch.Tensor, x: torch.Tensor, w_shape, stride: int, pad: i
     return gw[:, :kh * kw * C].reshape(Cout, kh, kw, C).permute(0, 3, 1, 2)
 
 
-# --------------------------------------------------------------------------------------------- pooling (NHWC kernels, conv_sm100.cu)
+# --------------------------------------------------------------------------------------------- pooling (NHWC kernels, conv_sm90.cu)
 def pool_native_ok(x: torch.Tensor) -> bool:
     return CONV_NATIVE and x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 4 and x.shape[1] % 8 == 0 and x.numel() > 0
 

@@ -1,4 +1,4 @@
-"""Fused attention op wrappers (kernels in csrc/attention_sm100.cu).
+"""Fused attention op wrappers (kernels in csrc/attention_sm90.cu).
 
 Tensors use the "bshd" convention: q/k/v are views [B, S, H, D] (arbitrary batch/seq/head strides, D
 contiguous) — typically slices of the fused qkv projection output [B, S, H, 3, D] (heads-major); the output is a
@@ -10,7 +10,7 @@ import math
 
 import torch
 
-_HD = 64   # head dim of the tcgen05 kernels (attention_sm100.cu)
+_HD = 64   # head dim of the wgmma kernels (attention_sm90.cu)
 
 
 def _can_pad(S: int, D: int, causal: bool) -> bool:
@@ -55,7 +55,7 @@ def attention_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: floa
             qp, kp, vp = (_pad_sd(t, S, D) for t in (q, k, v))
             o, lse = attention_fwd(qp, kp, vp, scale, causal)
             return o[:, :S, :, :D].contiguous(), lse[:, :, :S].contiguous()
-        o, lse, _ = _ref_fwd(q, k, v, scale, causal)   # shapes the tcgen05 kernel does not cover: plain torch math
+        o, lse, _ = _ref_fwd(q, k, v, scale, causal)   # shapes the wgmma kernel does not cover: plain torch math
         return o, lse
     from . import lib, _check, _count, _stream
     assert q.dtype == torch.bfloat16 and q.stride(3) == 1
@@ -125,7 +125,7 @@ def _native_ring(*ts: torch.Tensor) -> bool:
 def attn_merge_(o_acc: torch.Tensor, lse_acc: torch.Tensor, lse_out: torch.Tensor, o_j: torch.Tensor, lse_j: torch.Tensor,
                 first: bool) -> torch.Tensor:
     """Log-sum-exp merge of one block's partial attention (o_j [B,L,H,D], lse_j [B,H,L]) into the running fp32 pair
-    (o_acc in place; the merged log-sum-exp goes to `lse_out`, which is returned).  One kernel (elementwise_sm100.cu
+    (o_acc in place; the merged log-sum-exp goes to `lse_out`, which is returned).  One kernel (elementwise_sm90.cu
     attn_merge_kernel); plain torch math on CPU."""
     B, L, H, D = o_j.shape
     if o_j.dtype == torch.bfloat16 and _native_ring(o_j, o_acc, lse_acc, lse_out, lse_j):

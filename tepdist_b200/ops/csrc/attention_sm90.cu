@@ -1,0 +1,534 @@
+// Fused (flash) attention for sm_90a, head_dim 64, bf16, with wgmma.mma_async on register accumulators.
+// Forward, one CTA per (128-query block, batch, head): two warpgroups own 64 query rows each, a producer warp streams K / V
+// tiles through a TMA + mbarrier ring.
+//   S = Q K^T            wgmma m64n128k16 (A = Q, B = K, both K-major in smem)        -> registers
+//   P = online softmax   in registers (quad shuffles for the row max / sum)
+//   O += P V             wgmma m64n64k16 with A = P from registers (the S fragment repacked to bf16), B = V MN-major
+// Q/K/V are read straight out of the fused qkv projection buffer [B, S, H, 3, D] (heads-major) with 4-D TMA maps
+// (no head-split transposes), O is written as [B, S, H, D] so it feeds the output projection GEMM.
+// The reference gets attention from XLA-fused batched dots + softmax fusions (SURVEY Appendix C);
+// this kernel is the H100-native replacement.
+#include "sm90_ptx.cuh"
+#include "launch.cuh"
+#include <math.h>
+#include <stdio.h>
+
+using namespace sm90;
+
+namespace {
+
+constexpr int HD = 64;        // head dim
+constexpr int BQ = 128;       // query rows per forward CTA
+constexpr int BKV = 128;      // kv rows per forward iteration / per backward CTA
+constexpr int KV_STAGES = 3;
+constexpr int THREADS = 288;  // warps 0..7: two compute warpgroups, warp 8: TMA producer
+
+constexpr int TILE_BYTES = 128 * HD * 2;  // 16 KB: a [128 x 64] bf16 tile (one SW128 chunk)
+constexpr int SM_Q = 0;
+constexpr int SM_K = SM_Q + TILE_BYTES;
+constexpr int SM_V = SM_K + KV_STAGES * TILE_BYTES;
+constexpr int SM_BAR = SM_V + KV_STAGES * TILE_BYTES;
+constexpr int FWD_SMEM = SM_BAR + 256 + 1024;
+
+struct AttnFwdParams {
+  void* O;      // bf16 [B, S, H, D]
+  float* lse;   // fp32 [B, H, S]   (natural-log domain, scaled scores)
+  int B, H, S, causal;
+  float scale_log2;  // softmax scale * log2(e)
+  float scale;
+};
+
+__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+__global__ void __launch_bounds__(THREADS, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                const __grid_constant__ CUtensorMap tmap_v, const AttnFwdParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM_BAR);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;               // [KV_STAGES]
+  uint64_t* kv_empty = bars + 1 + KV_STAGES;  // [KV_STAGES]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nq = p.S / BQ;
+  const int BH = p.B * p.H;
+  const int qi = p.causal ? nq - 1 - (int)(blockIdx.x / BH) : (int)(blockIdx.x / BH);  // longest causal rows first
+  const int bh = blockIdx.x % BH;
+  const int b = bh / p.H, h = bh % p.H;
+  const int nkv = p.causal ? qi + 1 : p.S / BKV;
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tmap_q);
+    tma_prefetch_desc(&tmap_k);
+    tma_prefetch_desc(&tmap_v);
+    mbar_init(q_full, 1);
+    for (int s = 0; s < KV_STAGES; ++s) {
+      mbar_init(&kv_full[s], 1);
+      mbar_init(&kv_empty[s], 2);   // one arrival per compute warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (warp == 8) {
+    if (lane == 0) {
+      mbar_expect_tx(q_full, TILE_BYTES);
+      tma_load_4d(smem + SM_Q, &tmap_q, q_full, 0, qi * BQ, h, b);
+      for (int j = 0; j < nkv; ++j) {
+        const int st = j % KV_STAGES;
+        mbar_wait(&kv_empty[st], ((j / KV_STAGES) & 1) ^ 1);
+        mbar_expect_tx(&kv_full[st], 2 * TILE_BYTES);
+        tma_load_4d(smem + SM_K + st * TILE_BYTES, &tmap_k, &kv_full[st], 0, j * BKV, h, b);
+        tma_load_4d(smem + SM_V + st * TILE_BYTES, &tmap_v, &kv_full[st], 0, j * BKV, h, b);
+      }
+    }
+    pdl_trigger();
+    return;
+  }
+
+  const int wg = warp >> 2;
+  const int g = lane >> 2, q = lane & 3;
+  const int row0 = wg * 64 + (warp & 3) * 16 + g;   // query row (in the tile) of fragment rows e < 2; +8 for e >= 2
+  const uint32_t sq = smem_u32(smem + SM_Q) + wg * 64 * 128;
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nkv; ++j) {
+    const int st = j % KV_STAGES;
+    mbar_wait(&kv_full[st], (j / KV_STAGES) & 1);
+    const uint32_t sk = smem_u32(smem + SM_K + st * TILE_BYTES), sv = smem_u32(smem + SM_V + st * TILE_BYTES);
+    float s[64];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_m64n128k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sq + k * 32, 0, 1024), make_smem_desc_sw128(sk + k * 32, 0, 1024),
+                                     k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    const bool diag = p.causal && j == qi;
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int r = row0 + hr * 8;
+      float mx = m[hr];
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int idx = 4 * jj + 2 * hr + e;
+          float x = s[idx] * p.scale_log2;
+          if (diag && 8 * jj + 2 * q + e > r) x = -INFINITY;
+          s[idx] = x;
+          mx = fmaxf(mx, x);
+        }
+      }
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float alpha = exp2f(m[hr] - mx);
+      m[hr] = mx;
+      float sum = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int idx = 4 * jj + 2 * hr + e;
+          const float pv = exp2f(s[idx] - mx);
+          s[idx] = pv;
+          sum += pv;
+        }
+      }
+      l[hr] = l[hr] * alpha + sum;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        o[4 * jj + 2 * hr] *= alpha;
+        o[4 * jj + 2 * hr + 1] *= alpha;
+      }
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      uint32_t a[4];
+      frag_a_from_acc(s, kk, a);
+      wgmma_m64n64k16_bf16_rs<1>(o, a, make_smem_desc_sw128(sv + kk * 16 * 128, 8192, 1024), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[st]);
+  }
+  pdl_trigger();
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    float lsum = l[hr];
+    lsum += __shfl_xor_sync(0xffffffffu, lsum, 1);
+    lsum += __shfl_xor_sync(0xffffffffu, lsum, 2);
+    const float inv = 1.f / lsum;
+    const int row = qi * BQ + row0 + hr * 8;
+    __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.O) + (((size_t)b * p.S + row) * p.H + h) * HD;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+      *reinterpret_cast<uint32_t*>(op + 8 * jj + 2 * q) = pack_bf16x2(o[4 * jj + 2 * hr] * inv, o[4 * jj + 2 * hr + 1] * inv);
+    if (q == 0) p.lse[((size_t)b * p.H + h) * p.S + row] = (m[hr] + log2f(lsum)) * 0.6931471805599453f;
+  }
+}
+
+// =====================================================================================================
+// Backward.  One CTA per (128-row kv block j, batch, head); two warpgroups own 64 kv rows each and loop over 64-row query
+// blocks i (those that see block j when causal), streamed by a producer warp.  Per warpgroup and block:
+//   S^T = K Q^T, dP^T = V dO^T                      wgmma m64n64k16, both operands K-major in smem
+//   P^T = exp2(S^T c - lse), dS^T = P^T (dP^T - delta)          in registers
+//   dV += P^T dO, dK += dS^T Q                      wgmma with A from registers, B (dO / Q) MN-major in smem
+//   dQ  = dS K over this warpgroup's 64 kv rows      dS^T goes through smem (read as an MN-major A operand) ->
+//                                                   fp32 red.add into dq_acc (summed over kv blocks / warpgroups)
+// =====================================================================================================
+constexpr int BQB = 64;                          // query rows per backward iteration
+constexpr int QB_BYTES = BQB * HD * 2;           // 8 KB
+constexpr int Q_STAGES = 3;
+constexpr int SB_K = 0;
+constexpr int SB_V = SB_K + TILE_BYTES;
+constexpr int SB_DS = SB_V + TILE_BYTES;         // dS^T [128 kv][64 q] bf16, SW128
+constexpr int SB_Q = SB_DS + TILE_BYTES;         // [Q_STAGES]
+constexpr int SB_DO = SB_Q + Q_STAGES * QB_BYTES;
+constexpr int SB_BAR = SB_DO + Q_STAGES * QB_BYTES;
+constexpr int BWD_SMEM = SB_BAR + 256 + 1024;
+
+struct AttnBwdParams {
+  const float* lse;    // [B,H,S]
+  const float* delta;  // [B,H,S]
+  float* dq_acc;       // fp32 [B,S,H,D] (zero-initialised)
+  void* dk;            // bf16, strided [B,S,H,D] view
+  void* dv;
+  long long dstride_b, dstride_s, dstride_h;
+  int B, H, S, causal;
+  float scale_log2, scale;
+};
+
+__global__ void __launch_bounds__(THREADS, 1)
+attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
+                const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
+                const AttnBwdParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SB_BAR);
+  uint64_t* kv_full = bars;
+  uint64_t* q_full = bars + 1;              // [Q_STAGES]
+  uint64_t* q_empty = bars + 1 + Q_STAGES;  // [Q_STAGES]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int BH = p.B * p.H;
+  const int j = (int)(blockIdx.x / BH);  // kv block; small j = most work, scheduled first
+  const int bh = blockIdx.x % BH;
+  const int b = bh / p.H, h = bh % p.H;
+  const int nqb = p.S / BQB;
+  const int i0 = p.causal ? j * (BKV / BQB) : 0;
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tmap_q);
+    tma_prefetch_desc(&tmap_k);
+    tma_prefetch_desc(&tmap_v);
+    tma_prefetch_desc(&tmap_do);
+    mbar_init(kv_full, 1);
+    for (int s = 0; s < Q_STAGES; ++s) {
+      mbar_init(&q_full[s], 1);
+      mbar_init(&q_empty[s], 2);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (warp == 8) {
+    if (lane == 0) {
+      mbar_expect_tx(kv_full, 2 * TILE_BYTES);
+      tma_load_4d(smem + SB_K, &tmap_k, kv_full, 0, j * BKV, h, b);
+      tma_load_4d(smem + SB_V, &tmap_v, kv_full, 0, j * BKV, h, b);
+      for (int i = i0, it = 0; i < nqb; ++i, ++it) {
+        const int st = it % Q_STAGES;
+        mbar_wait(&q_empty[st], ((it / Q_STAGES) & 1) ^ 1);
+        mbar_expect_tx(&q_full[st], 2 * QB_BYTES);
+        tma_load_4d(smem + SB_Q + st * QB_BYTES, &tmap_q, &q_full[st], 0, i * BQB, h, b);
+        tma_load_4d(smem + SB_DO + st * QB_BYTES, &tmap_do, &q_full[st], 0, i * BQB, h, b);
+      }
+    }
+    pdl_trigger();
+    return;
+  }
+
+  const int wg = warp >> 2;
+  const int g = lane >> 2, q = lane & 3;
+  const int r0 = (warp & 3) * 16 + g;      // fragment row inside the warpgroup's 64 rows (+8 for e >= 2)
+  const uint32_t sk = smem_u32(smem + SB_K) + wg * 64 * 128, sv = smem_u32(smem + SB_V) + wg * 64 * 128;
+  uint8_t* ds_tile = smem + SB_DS + wg * 64 * 128;   // this warpgroup's 64 kv rows of dS^T
+  const uint32_t sds = smem_u32(ds_tile);
+  const float* lse_bh = p.lse + ((size_t)b * p.H + h) * p.S;
+  const float* delta_bh = p.delta + ((size_t)b * p.H + h) * p.S;
+  float dv[32], dk[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  mbar_wait(kv_full, 0);
+  for (int i = i0, it = 0; i < nqb; ++i, ++it) {
+    const int st = it % Q_STAGES;
+    mbar_wait(&q_full[st], (it / Q_STAGES) & 1);
+    const uint32_t sq = smem_u32(smem + SB_Q + st * QB_BYTES), sdo = smem_u32(smem + SB_DO + st * QB_BYTES);
+    float s[32], dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_m64n64k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sk + k * 32, 0, 1024), make_smem_desc_sw128(sq + k * 32, 0, 1024),
+                                    k > 0 ? 1u : 0u);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_m64n64k16_bf16_ss<0, 0>(dp, make_smem_desc_sw128(sv + k * 32, 0, 1024), make_smem_desc_sw128(sdo + k * 32, 0, 1024),
+                                    k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    fence_regs(dp);
+    const bool masked = p.causal && i * BQB < j * BKV + BKV;   // query block overlaps the kv block
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+      for (int e1 = 0; e1 < 2; ++e1) {
+        const int qt = 8 * jj + 2 * q + e1;
+        const float L = __ldg(lse_bh + i * BQB + qt) * 1.4426950408889634f;
+        const float dl = __ldg(delta_bh + i * BQB + qt);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int idx = 4 * jj + 2 * hr + e1;
+          float pv = exp2f(s[idx] * p.scale_log2 - L);
+          if (masked && i * BQB + qt < j * BKV + wg * 64 + r0 + 8 * hr) pv = 0.f;
+          s[idx] = pv;
+          dp[idx] = pv * (dp[idx] - dl);
+        }
+      }
+    }
+    // dS^T -> smem: element (kv row r, query column c) at byte r * 128 + 2c of the SW128 tile (16-byte chunk index XOR r % 8)
+    named_bar_sync(1 + wg, 128);   // this warpgroup's previous dQ MMA has finished reading the tile
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int r = r0 + 8 * hr;
+        const uint32_t byte = r * 128 + (8 * jj + 2 * q) * 2;
+        *reinterpret_cast<uint32_t*>(ds_tile + (byte ^ ((r & 7) << 4))) = pack_bf16x2(dp[4 * jj + 2 * hr], dp[4 * jj + 2 * hr + 1]);
+      }
+    }
+    fence_proxy_async();
+    named_bar_sync(1 + wg, 128);
+    float dq[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t a[4];
+      frag_a_from_acc(s, kk, a);
+      wgmma_m64n64k16_bf16_rs<1>(dv, a, make_smem_desc_sw128(sdo + kk * 16 * 128, 8192, 1024), 1u);
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      uint32_t a[4];
+      frag_a_from_acc(dp, kk, a);
+      wgmma_m64n64k16_bf16_rs<1>(dk, a, make_smem_desc_sw128(sq + kk * 16 * 128, 8192, 1024), 1u);
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+      wgmma_m64n64k16_bf16_ss<1, 1>(dq, make_smem_desc_sw128(sds + kk * 16 * 128, 8192, 1024),
+                                    make_smem_desc_sw128(sk + kk * 16 * 128, 8192, 1024), kk > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(dv);
+    fence_regs(dk);
+    fence_regs(dq);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&q_empty[st]);
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int row = i * BQB + r0 + 8 * hr;
+      float* dqp = p.dq_acc + (((size_t)b * p.S + row) * p.H + h) * HD;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dqp + 8 * jj + 2 * q), "f"(dq[4 * jj + 2 * hr] * p.scale),
+                     "f"(dq[4 * jj + 2 * hr + 1] * p.scale)
+                     : "memory");
+    }
+  }
+  pdl_trigger();
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = j * BKV + wg * 64 + r0 + 8 * hr;
+    const size_t off = (size_t)b * p.dstride_b + (size_t)row * p.dstride_s + (size_t)h * p.dstride_h;
+    __nv_bfloat16* dkp = reinterpret_cast<__nv_bfloat16*>(p.dk) + off;
+    __nv_bfloat16* dvp = reinterpret_cast<__nv_bfloat16*>(p.dv) + off;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      *reinterpret_cast<uint32_t*>(dkp + 8 * jj + 2 * q) = pack_bf16x2(dk[4 * jj + 2 * hr] * p.scale, dk[4 * jj + 2 * hr + 1] * p.scale);
+      *reinterpret_cast<uint32_t*>(dvp + 8 * jj + 2 * q) = pack_bf16x2(dv[4 * jj + 2 * hr], dv[4 * jj + 2 * hr + 1]);
+    }
+  }
+}
+
+// delta[b,h,s] = sum_d dO * O ; 8 lanes per (b, s, h) row of 64 elements (one 16-byte load per lane and tensor).
+__global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ dO, const __nv_bfloat16* __restrict__ O,
+                                  float* __restrict__ delta, int B, int S, int H) {
+  const long long gid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  const long long row = gid >> 3;
+  const int sub = (int)(gid & 7);
+  pdl_wait();
+  if (row >= (long long)B * S * H) return;
+  const int hh = row % H, s = (row / H) % S, bb = row / ((long long)H * S);
+  const uint4 a = __ldg(reinterpret_cast<const uint4*>(dO + row * HD) + sub);
+  const uint4 c = __ldg(reinterpret_cast<const uint4*>(O + row * HD) + sub);
+  const __nv_bfloat162* ha = reinterpret_cast<const __nv_bfloat162*>(&a);
+  const __nv_bfloat162* hc = reinterpret_cast<const __nv_bfloat162*>(&c);
+  float v = 0.f;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    float2 fa = __bfloat1622float2(ha[i]), fc = __bfloat1622float2(hc[i]);
+    v += fa.x * fc.x + fa.y * fc.y;
+  }
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  v += __shfl_xor_sync(0xffffffffu, v, 2);
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  if (sub == 0) delta[((size_t)bb * H + hh) * S + s] = v;
+}
+
+// dq (bf16, strided) = dq_acc (fp32 contiguous [B,S,H,D])
+// (the accumulator is zeroed again on the way out, so the persistent workspace never needs a separate memset)
+__global__ void attn_dq_cast_kernel(float* __restrict__ acc, __nv_bfloat16* __restrict__ dq, int B, int S, int H,
+                                    long long sb, long long ss, long long sh) {
+  const size_t n8 = (size_t)B * S * H * (HD / 8);
+  pdl_wait();
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n8; i += (size_t)gridDim.x * blockDim.x) {
+    const int v = i % (HD / 8);
+    size_t r = i / (HD / 8);
+    const int hh = r % H; r /= H;
+    const int s = r % S;
+    const int bb = r / S;
+    const float4 x = reinterpret_cast<const float4*>(acc)[i * 2], y = reinterpret_cast<const float4*>(acc)[i * 2 + 1];
+    uint4 u;
+    u.x = pack_bf16x2(x.x, x.y); u.y = pack_bf16x2(x.z, x.w); u.z = pack_bf16x2(y.x, y.y); u.w = pack_bf16x2(y.z, y.w);
+    *reinterpret_cast<uint4*>(dq + (size_t)bb * sb + (size_t)s * ss + (size_t)hh * sh + v * 8) = u;
+    reinterpret_cast<float4*>(acc)[i * 2] = make_float4(0.f, 0.f, 0.f, 0.f);
+    reinterpret_cast<float4*>(acc)[i * 2 + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
+                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                  CUtensorMapFloatOOBfill);
+EncodeTiledFn encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  if (!fn) {
+    void* ptr = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) != cudaSuccess) return nullptr;
+    fn = reinterpret_cast<EncodeTiledFn>(ptr);
+  }
+  return fn;
+}
+
+}  // namespace
+
+// 4-D map over a [B, S, H, D]-addressable bf16 tensor given element strides; box = {64, box_rows, 1, 1}.
+extern "C" int tepd_make_tmap_bshd(CUtensorMap* out, const void* ptr, int B, int S, int H, int D, long long stride_b,
+                                   long long stride_s, long long stride_h, int box_rows) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) return -1;
+  cuuint64_t dims[4] = {(cuuint64_t)D, (cuuint64_t)S, (cuuint64_t)H, (cuuint64_t)B};
+  cuuint64_t strides[3] = {(cuuint64_t)stride_s * 2, (cuuint64_t)stride_h * 2, (cuuint64_t)stride_b * 2};
+  cuuint32_t box[4] = {64, (cuuint32_t)box_rows, 1, 1};
+  cuuint32_t es[4] = {1, 1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : (int)r;
+}
+
+// q, k, v: bf16 pointers addressed as [B, S, H, D] with the given element strides (shared by q/k/v).
+extern "C" int tepd_attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, int B, int H, int S, int D,
+                             float scale, int causal, long long stride_b, long long stride_s, long long stride_h,
+                             void* stream) {
+  if (D != HD || S % 128 != 0) return -2;
+  CUtensorMap tq, tk, tv;
+  int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, D, stride_b, stride_s, stride_h, BQ);
+  if (rc) return 100 + rc;
+  rc = tepd_make_tmap_bshd(&tk, k, B, S, H, D, stride_b, stride_s, stride_h, BKV);
+  if (rc) return 200 + rc;
+  rc = tepd_make_tmap_bshd(&tv, v, B, S, H, D, stride_b, stride_s, stride_h, BKV);
+  if (rc) return 300 + rc;
+  static bool cfg = false;
+  if (!cfg) {
+    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM);
+    if (e != cudaSuccess) return (int)e;
+    cfg = true;
+  }
+  AttnFwdParams p;
+  p.O = o; p.lse = (float*)lse; p.B = B; p.H = H; p.S = S; p.causal = causal;
+  p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
+  return (int)tepd::launch(attn_fwd_kernel, dim3((S / BQ) * B * H), dim3(THREADS), FWD_SMEM, reinterpret_cast<cudaStream_t>(stream),
+                           tq, tk, tv, p);
+}
+
+// do, o: contiguous [B,S,H,D]; q/k/v strided views; dq/dk/dv strided views (shared strides).
+extern "C" int tepd_attn_bwd(const void* dO, const void* q, const void* k, const void* v, const void* o, const void* lse,
+                             void* dq_acc, void* dq, void* dk, void* dv, int B, int H, int S, int D, float scale,
+                             int causal, long long stride_b, long long stride_s, long long stride_h, long long dstride_b,
+                             long long dstride_s, long long dstride_h, void* stream) {
+  if (D != HD || S % 128 != 0) return -2;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CUtensorMap tq, tk, tv, tdo;
+  int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, D, stride_b, stride_s, stride_h, BQB);
+  if (rc) return 100 + rc;
+  rc = tepd_make_tmap_bshd(&tk, k, B, S, H, D, stride_b, stride_s, stride_h, BKV);
+  if (rc) return 200 + rc;
+  rc = tepd_make_tmap_bshd(&tv, v, B, S, H, D, stride_b, stride_s, stride_h, BKV);
+  if (rc) return 300 + rc;
+  rc = tepd_make_tmap_bshd(&tdo, dO, B, S, H, D, (long long)S * H * D, (long long)H * D, D, BQB);
+  if (rc) return 400 + rc;
+  static float* delta_buf = nullptr;
+  static size_t delta_cap = 0;
+  const size_t need = (size_t)B * H * S;
+  if (need > delta_cap) {
+    if (delta_buf) cudaFree(delta_buf);
+    if (cudaMalloc(&delta_buf, need * sizeof(float)) != cudaSuccess) return -5;
+    delta_cap = need;
+  }
+  {
+    const long long rows = (long long)B * S * H;
+    cudaError_t le = tepd::launch(attn_delta_kernel, dim3((unsigned)((rows * 8 + 255) / 256)), dim3(256), 0, st,
+                                  (const __nv_bfloat16*)dO, (const __nv_bfloat16*)o, delta_buf, B, S, H);
+    if (le != cudaSuccess) return (int)le;
+  }
+  // persistent, self-clearing fp32 dQ accumulator (used when the caller passes no buffer)
+  static float* dq_ws = nullptr;
+  static size_t dq_cap = 0;
+  if (dq_acc == nullptr) {
+    const size_t needq = (size_t)B * S * H * HD;
+    if (needq > dq_cap) {
+      if (dq_ws) cudaFree(dq_ws);
+      if (cudaMalloc(&dq_ws, needq * sizeof(float)) != cudaSuccess) return -6;
+      cudaMemsetAsync(dq_ws, 0, needq * sizeof(float), st);
+      dq_cap = needq;
+    }
+    dq_acc = dq_ws;
+  }
+  static bool cfg = false;
+  if (!cfg) {
+    cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
+    if (e != cudaSuccess) return (int)e;
+    cfg = true;
+  }
+  AttnBwdParams p;
+  p.lse = (const float*)lse; p.delta = delta_buf; p.dq_acc = (float*)dq_acc; p.dk = dk; p.dv = dv;
+  p.dstride_b = dstride_b; p.dstride_s = dstride_s; p.dstride_h = dstride_h;
+  p.B = B; p.H = H; p.S = S; p.causal = causal; p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
+  cudaError_t le = tepd::launch(attn_bwd_kernel, dim3((S / BKV) * B * H), dim3(THREADS), BWD_SMEM, st, tq, tk, tv, tdo, p);
+  if (le != cudaSuccess) return (int)le;
+  return (int)tepd::launch(attn_dq_cast_kernel, dim3(tepd::num_sms() * 4), dim3(256), 0, st, (float*)dq_acc, (__nv_bfloat16*)dq, B, S, H,
+                           dstride_b, dstride_s, dstride_h);
+}

@@ -1,0 +1,701 @@
+// Persistent warp-specialised GEMM for sm_90a: TMA -> smem (SWIZZLE_128B, multi-stage mbarrier ring) -> wgmma.mma_async
+// into register accumulators of two consumer warpgroups -> epilogue from the accumulator fragments (bias / GELU /
+// residual / fp32 split-K or stream-K reduction fused).  bf16 operands, and e4m3 operands for the MoE expert GEMMs
+// (tepd_gemm_fp8).  This is the device-op layer that replaces the reference's cuBLAS GemmThunk
+// (reference: tensorflow/compiler/xla/service/gpu/gemm_thunk.cc, SURVEY §2.H K8).
+//
+//   D[b, M, N] = epilogue( alpha * A[b] (M x K)  *  B[b] (K x N) )
+//
+// Operand storage is described per operand by a "major" flag:
+//   A K-major : memory [b, M, K] (K contiguous)       A MN-major: memory [b, K, M] (M contiguous)
+//   B K-major : memory [b, N, K] (K contiguous)       B MN-major: memory [b, K, N] (N contiguous)
+// which covers forward (x @ W^T), dgrad (dy @ W) and wgrad (dy^T @ x) without any transposes.
+#include "sm90_ptx.cuh"
+#include "launch.cuh"
+#include <stdio.h>
+#include <map>
+#include <mutex>
+#include <utility>
+
+using namespace sm90;
+
+namespace {
+
+constexpr int BLOCK_M = 128;
+constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row (128 e4m3 elements for the fp8 kernel)
+constexpr int NUM_THREADS = 288;  // warps 0..7: two consumer warpgroups, warp 8: TMA producer
+
+struct GemmParams {
+  int M, N, K, batch;
+  int m_blocks, n_blocks, k_blocks, split_k;
+  long long ldd, stride_d;       // output leading dim / batch stride (elements)
+  long long ld_res, stride_res;  // residual
+  void* D;
+  const void* bias;      // fp32 [N] or nullptr
+  const void* residual;  // bf16 [b, M, N] or nullptr
+  float alpha;
+  int out_fp32;    // 0: bf16 output, 1: fp32 output
+  int accumulate;  // 1: red.add into fp32 output (split-K / gradient accumulation)
+  int act;         // 0 none, 1 tanh-GELU, 2 multiply by GELU'(aux)  (fused gelu backward on a dgrad GEMM)
+  int bias_bf16;
+  void* D2;        // act 1: when set, D receives the pre-activation and D2 the activated value (saved for backward)
+  const void* aux; // act 2: bf16 [b, M, N] pre-activation
+  float* sk_ws;        // stream-K fix-up workspace: [CTA][BLOCK_M][BLOCK_N] fp32 partial tiles
+  unsigned* sk_cnt;    // per CTA: 1 = its partial tile is complete (reset to 0 by the consumer)
+  const float* row_scale;  // fp8: per-row activation scale [b, M] (nullptr: none); multiplied with w_scale[b]
+  const float* w_scale;
+  long long bias_stride;   // bias batch stride (elements): 0 = one bias for every batch
+  int stream_k;    // > 0: stream-K -- CTA c owns the contiguous range [c, c+1) * stream_k of the (tile, k-block) iteration
+                   // space and flushes its accumulator with red.add at every tile boundary (fp32 accumulate outputs only):
+                   // every SM gets the same number of k-blocks whatever the tile count (no wave quantisation)
+};
+
+// One unit of work for a CTA: k-blocks [kb0, kb1) of output tile (m_blk, n_blk, b).  `lead` = this unit holds k-block 0
+// (it adds bias / residual).  Data-parallel + split-K: cursor walks tile indices blockIdx.x, +gridDim.x, ...;
+// stream-K: cursor walks this CTA's iteration range and a unit ends at the tile boundary or at the end of the range.
+struct Work {
+  int m_blk, n_blk, b, kb0, kb1;
+  bool lead;
+};
+__device__ __forceinline__ void work_range(const GemmParams& p, int& cursor, int& end) {
+  if (p.stream_k > 0) {
+    const long long total = (long long)p.m_blocks * p.n_blocks * p.batch * p.k_blocks;
+    const long long c0 = (long long)blockIdx.x * p.stream_k;
+    cursor = (int)(c0 < total ? c0 : total);
+    end = (int)(c0 + p.stream_k < total ? c0 + p.stream_k : total);
+  } else {
+    cursor = blockIdx.x;
+    end = p.m_blocks * p.n_blocks * p.batch * p.split_k;
+  }
+}
+__device__ __forceinline__ void next_work(const GemmParams& p, int& cursor, int end, Work& w) {
+  int t;
+  if (p.stream_k > 0) {
+    t = cursor / p.k_blocks;
+    w.kb0 = cursor - t * p.k_blocks;
+    w.kb1 = min(p.k_blocks, w.kb0 + (end - cursor));
+    w.lead = w.kb0 == 0;
+    cursor += w.kb1 - w.kb0;
+  } else {
+    t = cursor;
+    cursor += gridDim.x;
+  }
+  w.m_blk = t % p.m_blocks; t /= p.m_blocks;
+  w.n_blk = t % p.n_blocks; t /= p.n_blocks;
+  w.b = t % p.batch;
+  if (p.stream_k <= 0) {
+    const int split = t / p.batch;
+    const int per = (p.k_blocks + p.split_k - 1) / p.split_k;
+    w.kb0 = split * per;
+    w.kb1 = min(p.k_blocks, w.kb0 + per);
+    w.lead = split == 0;
+  }
+}
+
+// Peer-memory fusion (tensor parallel):
+//   mode 1  GEMM -> reduce-scatter : output rows [r*rows_per_owner, (r+1)*rows_per_owner) are reduced into rank r's fp32
+//           buffer with red.add over NVLink straight from the epilogue (no separate collective, overlaps tile by tile)
+//   mode 2  all-gather -> GEMM     : A rows are fetched by TMA directly from the rank that owns them (peer-mapped shards)
+//   mode 3  GEMM -> reduce-scatter : partial rows are written as bf16 with plain 16-byte stores into slot [src rank] of the
+//           owner's staging buffer (no atomics on the wire); slot_reduce (comm_sm90.cu) sums the n slots on the owner
+//   mode 4  all-gather -> GEMM     : a concurrent copy kernel (p2p_gather_chunks) pulls the peers' shards into a local
+//           staging buffer chunk by chunk and publishes a flag per chunk; the TMA producer starts on the local shard and
+//           waits on a chunk's flag just before its first tile of that chunk, so the NVLink transfer hides under the MMAs
+// Peer tiles are walked chunk-major (own rows first, then rank+1's, ...), so at any moment the n ranks talk to n
+// different peers and mode 4 meets its chunks in the order the copy kernel delivers them.
+constexpr int MAX_PEERS = 8;
+struct PeerArgs {
+  int mode, n, rank, rows_per_owner;
+  void* out[MAX_PEERS];
+  const uint32_t* flags;  // mode 4: flags[owner] == *epoch once owner's rows are staged locally
+  const uint32_t* epoch;
+};
+
+__device__ __forceinline__ void peer_tile(const PeerArgs* pa, int m_blocks, int n_blocks, int tile, int& m_blk, int& n_blk) {
+  const int mpc = m_blocks / pa->n;  // m-blocks per owner chunk
+  const int per_chunk = mpc * n_blocks;
+  const int chunk = tile / per_chunk;
+  const int rem = tile - chunk * per_chunk;
+  n_blk = rem / mpc;
+  int owner = pa->rank + chunk;
+  if (owner >= pa->n) owner -= pa->n;
+  m_blk = owner * mpc + (rem - n_blk * mpc);
+}
+struct TmapArray {
+  CUtensorMap m[MAX_PEERS];
+};
+
+__device__ __forceinline__ float gelu_tanh_grad(float x) {
+  const float k0 = 0.7978845608028654f, k1 = 0.044715f;
+  float t;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(k0 * (x + k1 * x * x * x)));
+  return 0.5f * (1.0f + t) + 0.5f * x * (1.0f - t * t) * k0 * (1.0f + 3.0f * k1 * x * x);
+}
+__device__ __forceinline__ float gelu_tanh(float x) {
+  const float k0 = 0.7978845608028654f, k1 = 0.044715f;
+  float u = k0 * (x + k1 * x * x * x);
+  float t;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(u));
+  return 0.5f * x * (1.0f + t);
+}
+
+template <int BLOCK_N>
+struct Cfg {
+  static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
+  static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGES = (BLOCK_N == 256) ? 4 : 6;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+};
+
+__device__ __forceinline__ void st_bf16x2(void* p, float a, float b) { *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(a, b); }
+__device__ __forceinline__ float2 ld_bf16x2(const void* p) {
+  return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
+}
+
+// Epilogue math + store for two adjacent columns (col, col + 1) of one output row.  v0 / v1 already hold the scaled
+// accumulator.  N % 8 == 0 and col is even, so col < N covers both columns.
+template <bool PEER>
+__device__ __forceinline__ void epilogue_pair(float v0, float v1, const GemmParams& p, const PeerArgs* pa, int row, int col, int b,
+                                              bool add_bias, bool add_res) {
+  if (add_bias) {
+    if (p.bias_bf16) {
+      const float2 f = ld_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.bias) + (long long)b * p.bias_stride + col);
+      v0 += f.x; v1 += f.y;
+    } else {
+      const float2 f = __ldg(reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.bias) + (long long)b * p.bias_stride + col));
+      v0 += f.x; v1 += f.y;
+    }
+  }
+  const long long off = (long long)b * p.stride_d + (long long)row * p.ldd + col;
+  if (p.act == 1) {
+    if (p.D2 != nullptr) st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.D) + off, v0, v1);  // pre-activation for backward
+    v0 = gelu_tanh(v0); v1 = gelu_tanh(v1);
+  } else if (p.act == 2) {
+    const float2 f = ld_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.aux) + off);
+    v0 *= gelu_tanh_grad(f.x); v1 *= gelu_tanh_grad(f.y);
+  }
+  if (add_res) {
+    const float2 f = ld_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.residual) + (long long)b * p.stride_res +
+                               (long long)row * p.ld_res + col);
+    v0 += f.x; v1 += f.y;
+  }
+  if (!p.out_fp32) {
+    __nv_bfloat16* dp = reinterpret_cast<__nv_bfloat16*>(p.D2 != nullptr && p.act == 1 ? p.D2 : p.D) + off;
+    if constexpr (PEER) {
+      if (pa->mode == 3) {  // partial rows -> slot [my rank] of the owner's staging buffer (plain stores over NVLink)
+        const int owner = row / pa->rows_per_owner;
+        dp = reinterpret_cast<__nv_bfloat16*>(pa->out[owner]) +
+             ((long long)pa->rank * pa->rows_per_owner + (row - owner * pa->rows_per_owner)) * p.ldd + col;
+      }
+    }
+    st_bf16x2(dp, v0, v1);
+  } else if (!p.accumulate) {
+    *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.D) + off) = make_float2(v0, v1);
+  } else {
+    float* dp = reinterpret_cast<float*>(p.D) + off;
+    if constexpr (PEER) {
+      if (pa->mode == 1) {  // reduce-scatter: this row belongs to rank `owner`; add into ITS buffer over NVLink
+        const int owner = row / pa->rows_per_owner;
+        dp = reinterpret_cast<float*>(pa->out[owner]) + (long long)(row - owner * pa->rows_per_owner) * p.ldd + col;
+      }
+    }
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dp), "f"(v0), "f"(v1) : "memory");
+  }
+}
+
+// One k-block (BLOCK_K = 128 bytes of K) of this warpgroup's 64 x BLOCK_N accumulator: four wgmma k-steps per 128-column
+// half.  bf16 steps are k16, e4m3 steps k32: 32 bytes of K either way, so the descriptors advance alike.
+template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 128][64], uint32_t sa, uint32_t sb, int wg, bool first) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    uint64_t da;
+    if constexpr (!A_MN) da = make_smem_desc_sw128(sa + wg * 64 * 128 + k * 32, 0, 1024);
+    else                 da = make_smem_desc_sw128(sa + wg * 64 * BLOCK_K * 2 + k * 16 * 128, 64 * BLOCK_K * 2, 1024);
+#pragma unroll
+    for (int h = 0; h < BLOCK_N / 128; ++h) {
+      uint64_t db;
+      if constexpr (!B_MN) db = make_smem_desc_sw128(sb + h * 128 * 128 + k * 32, 0, 1024);
+      else                 db = make_smem_desc_sw128(sb + h * 2 * 64 * BLOCK_K * 2 + k * 16 * 128, 64 * BLOCK_K * 2, 1024);
+      const uint32_t scale_d = (first && k == 0) ? 0u : 1u;
+      if constexpr (FP8) wgmma_m64n128k32_e4m3_ss(acc[h], da, db, scale_d);
+      else               wgmma_m64n128k16_bf16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], da, db, scale_d);
+    }
+  }
+}
+
+// Warp roles: warps 0-7 = two consumer warpgroups (wgmma into registers, rows [64 wg, +64) of the 128-row tile, then the
+// epilogue straight from the accumulator fragments); warp 8 = TMA producer.
+template <int BLOCK_N, bool A_MN, bool B_MN, bool PEER, bool FP8>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmParams& p,
+                                          const PeerArgs* pa, const TmapArray* tmaps_a) {
+  using C = Cfg<BLOCK_N>;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + C::STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (warp == 8 && lane == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    for (int s = 0; s < C::STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);   // one arrival per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();      // everything above overlapped the previous kernel's tail; its outputs are visible from here on
+  pdl_trigger();   // persistent grid: the next kernel may be scheduled as these CTAs retire
+
+  if (warp == 8) {
+    // ===================== TMA producer =====================
+    if (elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      int peer_ready = -1;
+      (void)peer_ready;
+      int cursor, cend;
+      work_range(p, cursor, cend);
+      while (cursor < cend) {
+        const int tile = cursor;
+        Work w;
+        next_work(p, cursor, cend, w);
+        int m_blk = w.m_blk, n_blk = w.n_blk;
+        const int b = w.b, kb0 = w.kb0, kb1 = w.kb1;
+        const CUtensorMap* ta = &tmap_a;
+        int a_row = m_blk * BLOCK_M;
+        if constexpr (PEER) {
+          peer_tile(pa, p.m_blocks, p.n_blocks, tile, m_blk, n_blk);
+          a_row = m_blk * BLOCK_M;
+          if (pa->mode == 2) {
+            const int owner = a_row / pa->rows_per_owner;
+            ta = &tmaps_a->m[owner];
+            a_row -= owner * pa->rows_per_owner;
+          } else if (pa->mode == 4) {
+            const int owner = a_row / pa->rows_per_owner;
+            if (owner == pa->rank) {  // own shard: read it where it lives
+              a_row -= owner * pa->rows_per_owner;
+            } else {                  // staged copy of a peer's shard: wait until the copy kernel published it
+              ta = &tmaps_a->m[(pa->rank + 1) % pa->n];
+              if (owner != peer_ready) {
+                const uint32_t want = *reinterpret_cast<const volatile uint32_t*>(pa->epoch);
+                uint32_t got;
+                const long long t0 = clock64();
+                do {
+                  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(got) : "l"(pa->flags + owner) : "memory");
+                  if (got != want && clock64() - t0 > 4000000000LL) __trap();  // copy kernel never ran: fail loudly, don't hang
+                } while (got != want);
+                asm volatile("fence.proxy.async;" ::: "memory");
+                peer_ready = owner;
+              }
+            }
+          }
+        }
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * C::STAGE_BYTES;
+          uint8_t* sb = sa + C::A_BYTES;
+          mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
+          if constexpr (!A_MN) {
+            tma_load_3d(sa, ta, &full_bar[stage], kb * BLOCK_K * (FP8 ? 2 : 1), a_row, b);
+          } else {
+#pragma unroll
+            for (int j = 0; j < BLOCK_M / 64; ++j)
+              tma_load_3d(sa + j * (64 * BLOCK_K * 2), &tmap_a, &full_bar[stage],
+                          m_blk * BLOCK_M + j * 64, kb * BLOCK_K, b);
+          }
+          if constexpr (!B_MN) {
+            tma_load_3d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K * (FP8 ? 2 : 1), n_blk * BLOCK_N, b);
+          } else {
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 64; ++j)
+              tma_load_3d(sb + j * (64 * BLOCK_K * 2), &tmap_b, &full_bar[stage],
+                          n_blk * BLOCK_N + j * 64, kb * BLOCK_K, b);
+          }
+          if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers: MMA + epilogue =====================
+    const int wg = warp >> 2;                 // rows [64 wg, 64 wg + 64) of the tile
+    const int t128 = threadIdx.x & 127;
+    const int g = lane >> 2, q = lane & 3;
+    const int row_base = wg * 64 + (warp & 3) * 16 + g;   // + 8 for the second half of each fragment
+    int stage = 0;
+    uint32_t phase = 0;
+    int cursor, cend;
+    work_range(p, cursor, cend);
+    while (cursor < cend) {
+      const int tile = cursor;
+      Work w;
+      next_work(p, cursor, cend, w);
+      int m_blk = w.m_blk, n_blk = w.n_blk;
+      const int b = w.b;
+      const bool has_k = w.kb0 < w.kb1;
+      if constexpr (PEER) peer_tile(pa, p.m_blocks, p.n_blocks, tile, m_blk, n_blk);
+      float acc[BLOCK_N / 128][64];
+      int prev = -1;
+      for (int kb = w.kb0; kb < w.kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
+        wgmma_fence();
+        mma_kblock<BLOCK_N, A_MN, B_MN, FP8>(acc, sa, sa + C::A_BYTES, wg, kb == w.kb0);
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot may be refilled
+        if (prev >= 0 && t128 == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int h = 0; h < BLOCK_N / 128; ++h) fence_regs(acc[h]);
+      if (prev >= 0 && t128 == 0) mbar_arrive(&empty_bar[prev]);
+
+      const bool add_bias = p.bias != nullptr && w.lead;
+      const bool add_res = p.residual != nullptr && w.lead;
+      // stream-K units that cover only part of a tile's K range (outputs with a real epilogue): a unit that starts
+      // mid-tile (always a CTA's FIRST unit) stores its fp32 partial tile into workspace slot [blockIdx.x] and raises
+      // flag[blockIdx.x]; the unit that holds k-block 0 (always a CTA's LAST unit) is the finisher: it waits for the
+      // flags of the CTAs that follow it inside the tile, adds their partials to its own accumulator and runs the real
+      // epilogue.  Producers never wait and finish their part first, so the wait is short and cannot deadlock.
+      const bool sk_part = p.stream_k > 0 && !p.accumulate && !(w.kb0 == 0 && w.kb1 == p.k_blocks);
+      const bool sk_store = sk_part && w.kb0 > 0;
+      const bool sk_finish = sk_part && w.kb0 == 0;
+      int partner_end = 0;   // finisher: partners are CTAs blockIdx.x+1 .. partner_end-1
+      if (sk_finish) {
+        const int tile_end = tile + p.k_blocks;   // (cursor before next_work == first iteration of the tile)
+        partner_end = blockIdx.x + 1;
+        while (partner_end < (int)gridDim.x && partner_end * p.stream_k < tile_end) ++partner_end;
+        if (threadIdx.x == 0) {
+          for (int j = blockIdx.x + 1; j < partner_end; ++j) {
+            unsigned f;
+            const long long t0 = clock64();
+            do {
+              asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(f) : "l"(p.sk_cnt + j) : "memory");
+              if (f == 0u && clock64() - t0 > 4000000000LL) __trap();   // a partner never arrived: fail loudly
+            } while (f == 0u);
+          }
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+      }
+      if (has_k) {
+        const float* scale_rows = p.row_scale ? p.row_scale + (long long)b * p.M : nullptr;
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int row_in_tile = row_base + hr * 8;
+          const int row = m_blk * BLOCK_M + row_in_tile;
+          if (row >= p.M) continue;
+          float alpha = p.alpha;
+          if (scale_rows) alpha *= scale_rows[row] * p.w_scale[b];
+#pragma unroll
+          for (int h = 0; h < BLOCK_N / 128; ++h) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              const int cit = h * 128 + j * 8 + 2 * q;   // column inside the tile
+              const int col = n_blk * BLOCK_N + cit;
+              if (col >= p.N) continue;
+              float v0 = acc[h][4 * j + 2 * hr] * alpha, v1 = acc[h][4 * j + 2 * hr + 1] * alpha;
+              float* wp = p.sk_ws + ((long long)blockIdx.x * BLOCK_M + row_in_tile) * 256 + cit;
+              if (sk_store) {
+                *reinterpret_cast<float2*>(wp) = make_float2(v0, v1);
+                continue;
+              }
+              if (sk_finish) {
+                for (int jj = blockIdx.x + 1; jj < partner_end; ++jj) {
+                  float2 t;
+                  asm volatile("ld.global.cg.v2.f32 {%0,%1}, [%2];" : "=f"(t.x), "=f"(t.y)
+                               : "l"(p.sk_ws + ((long long)jj * BLOCK_M + row_in_tile) * 256 + cit));
+                  v0 += t.x; v1 += t.y;
+                }
+              }
+              epilogue_pair<PEER>(v0, v1, p, pa, row, col, b, add_bias, add_res);
+            }
+          }
+        }
+      }
+      if (sk_part) {
+        if (sk_store) __threadfence();
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (threadIdx.x == 0) {
+          if (sk_store) {
+            asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p.sk_cnt + blockIdx.x), "r"(1u) : "memory");
+          } else {
+            for (int j = blockIdx.x + 1; j < partner_end; ++j) p.sk_cnt[j] = 0u;   // consumed: clean for the next launch
+          }
+        }
+      }
+    }
+  }
+}
+
+template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const GemmParams p) {
+  gemm_body<BLOCK_N, A_MN, B_MN, false, FP8>(tmap_a, tmap_b, p, nullptr, nullptr);
+}
+
+template <int BLOCK_N, bool B_MN>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+gemm_bf16_peer_kernel(const __grid_constant__ TmapArray tmaps_a, const __grid_constant__ CUtensorMap tmap_b,
+                      const GemmParams p, const __grid_constant__ PeerArgs pa) {
+  gemm_body<BLOCK_N, false, B_MN, true, false>(tmaps_a.m[pa.rank], tmap_b, p, &pa, &tmaps_a);
+}
+
+// ------------------------------------------------------------------ host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
+                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                  CUtensorMapFloatOOBfill);
+
+EncodeTiledFn get_encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || !p) {
+      fprintf(stderr, "[tepdist] cuTensorMapEncodeTiled unavailable\n");
+      return nullptr;
+    }
+    fn = reinterpret_cast<EncodeTiledFn>(p);
+  }
+  return fn;
+}
+
+}  // namespace
+
+// 3-D bf16 tensor map: dims (inner, rows, batch); box (box_inner, box_rows, 1); SWIZZLE_128B.
+extern "C" int tepd_make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, long long inner, long long rows,
+                                      long long batch, long long ld_elems, long long batch_stride_elems,
+                                      int box_inner, int box_rows) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return -1;
+  cuuint64_t dims[3] = {(cuuint64_t)inner, (cuuint64_t)rows, (cuuint64_t)batch};
+  cuuint64_t strides[2] = {(cuuint64_t)ld_elems * 2, (cuuint64_t)(batch > 1 ? batch_stride_elems : rows * ld_elems) * 2};
+  cuuint32_t box[3] = {(cuuint32_t)box_inner, (cuuint32_t)box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? 0 : (int)r;
+}
+
+template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8 = false>
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int num_sms,
+                       cudaStream_t stream) {
+  using C = Cfg<BLOCK_N>;
+  auto kern = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, FP8>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    if (e != cudaSuccess) return (int)e;
+    configured = true;
+  }
+  int total = p.m_blocks * p.n_blocks * p.batch * p.split_k;
+  int grid = total < num_sms ? total : num_sms;
+  if (p.stream_k > 0) {
+    const long long iters = (long long)p.m_blocks * p.n_blocks * p.batch * p.k_blocks;
+    grid = (int)((iters + p.stream_k - 1) / p.stream_k);
+  }
+  return (int)tepd::launch(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, ta, tb, p);
+}
+
+// C ABI entry (called from Python via ctypes).  All leading dims / strides are in elements.
+extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void* bias, const void* residual,
+                              int M, int N, int K, int batch, long long lda, long long ldb, long long ldd,
+                              long long stride_a, long long stride_b, long long stride_d, long long ld_res,
+                              long long stride_res, int a_mn, int b_mn, int out_fp32, int accumulate, int act,
+                              int bias_bf16, float alpha, int split_k, int block_n, int num_sms, void* stream, void* D2,
+                              const void* aux) {
+  // K % 8 is a TMA row-pitch requirement of K-major operands only (MN-major operands have K as the outer dimension)
+  if (N % 8 != 0 || M <= 0 || (K % 8 != 0 && !(a_mn && b_mn))) return -2;
+  if ((D2 || aux) && out_fp32) return -5;
+  if ((a_mn && (M % 8)) || (accumulate && !out_fp32)) return -3;
+  GemmParams p;
+  p.M = M; p.N = N; p.K = K; p.batch = batch;
+  if (block_n != 128 && block_n != 256) block_n = (N % 256 == 0 || N > 1024) ? 256 : 128;
+  p.m_blocks = (M + BLOCK_M - 1) / BLOCK_M;
+  p.n_blocks = (N + block_n - 1) / block_n;
+  p.k_blocks = (K + BLOCK_K - 1) / BLOCK_K;
+  p.stream_k = 0; p.sk_ws = nullptr; p.sk_cnt = nullptr;
+  if (num_sms <= 0) num_sms = tepd::num_sms();
+  if (split_k < 0) {  // stream-K requested: equal k-block ranges per SM
+    const long long iters = (long long)p.m_blocks * p.n_blocks * batch * p.k_blocks;
+    long long per = (iters + num_sms - 1) / num_sms;
+    if (per < 4) per = 4;   // do not shred tiny problems into sub-4-k-block units
+    p.stream_k = (int)per;
+    split_k = 1;
+    if (!(out_fp32 && accumulate)) {
+      // outputs with a real epilogue: partial tiles travel through a per-device fp32 workspace (one slot per CTA);
+      // allocated once; flags are reset by their consumer.  GEMMs of one device must not run concurrently on two
+      // streams in this mode.
+      constexpr int kSlots = 160;
+      // pool of workspaces per device, all allocated at the first call (the executor's eager warm-up step, i.e. outside
+      // CUDA-graph capture); every stream is bound to one of them in order of first appearance (binding allocates nothing,
+      // so it may happen during capture), so stream-K GEMMs on up to kPool concurrent streams never share partial tiles
+      constexpr int kPool = 4;
+      struct SkWs { float* ws; unsigned* cnt; };
+      struct DevPool { bool ready = false; SkWs w[kPool]; std::map<void*, int> bound; int next = 0; };
+      static DevPool pools[16];
+      static std::mutex pool_mu;
+      int dev = 0;
+      cudaGetDevice(&dev);
+      if (num_sms + 1 > kSlots || dev >= 16) return -6;
+      SkWs w;
+      {
+        std::lock_guard<std::mutex> lk(pool_mu);
+        DevPool& dp = pools[dev];
+        if (!dp.ready) {
+          const size_t bytes = (size_t)kSlots * BLOCK_M * 256 * sizeof(float);
+          for (int i = 0; i < kPool; ++i) {
+            if (cudaMalloc(&dp.w[i].ws, bytes) != cudaSuccess) return -7;
+            if (cudaMalloc(&dp.w[i].cnt, kSlots * sizeof(unsigned)) != cudaSuccess) return -7;
+            cudaMemset(dp.w[i].ws, 0, bytes);
+            cudaMemset(dp.w[i].cnt, 0, kSlots * sizeof(unsigned));
+          }
+          cudaDeviceSynchronize();
+          dp.ready = true;
+        }
+        auto it = dp.bound.find(stream);
+        if (it == dp.bound.end()) it = dp.bound.emplace(stream, dp.next++ % kPool).first;
+        w = dp.w[it->second];
+      }
+      p.sk_ws = w.ws; p.sk_cnt = w.cnt;
+    }
+  }
+  if (split_k < 1) split_k = 1;
+  if (split_k > p.k_blocks) split_k = p.k_blocks;
+  if (split_k > 1) {
+    // make every split non-empty
+    int per = (p.k_blocks + split_k - 1) / split_k;
+    split_k = (p.k_blocks + per - 1) / per;
+    if (!(out_fp32 && accumulate)) return -4;
+  }
+  p.split_k = split_k;
+  p.ldd = ldd; p.stride_d = stride_d; p.ld_res = ld_res; p.stride_res = stride_res;
+  p.D = D; p.bias = bias; p.residual = residual; p.alpha = alpha;
+  p.out_fp32 = out_fp32; p.accumulate = accumulate; p.act = act; p.bias_bf16 = bias_bf16;
+  p.D2 = D2; p.aux = aux;
+  p.row_scale = nullptr; p.w_scale = nullptr; p.bias_stride = 0;
+
+  CUtensorMap ta, tb;
+  int rc;
+  if (!a_mn) rc = tepd_make_tmap_bf16_3d(&ta, A, K, M, batch, lda, stride_a, BLOCK_K, BLOCK_M);
+  else       rc = tepd_make_tmap_bf16_3d(&ta, A, M, K, batch, lda, stride_a, 64, BLOCK_K);
+  if (rc) return 100 + rc;
+  if (!b_mn) rc = tepd_make_tmap_bf16_3d(&tb, B, K, N, batch, ldb, stride_b, BLOCK_K, block_n);
+  else       rc = tepd_make_tmap_bf16_3d(&tb, B, N, K, batch, ldb, stride_b, 64, BLOCK_K);
+  if (rc) return 200 + rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+#define DISPATCH(BN)                                                                   \
+  if (!a_mn && !b_mn) return launch_gemm<BN, false, false>(ta, tb, p, num_sms, s);     \
+  if (!a_mn && b_mn) return launch_gemm<BN, false, true>(ta, tb, p, num_sms, s);       \
+  if (a_mn && !b_mn) return launch_gemm<BN, true, false>(ta, tb, p, num_sms, s);       \
+  return launch_gemm<BN, true, true>(ta, tb, p, num_sms, s);
+  if (block_n == 256) { DISPATCH(256) } else { DISPATCH(128) }
+#undef DISPATCH
+}
+
+
+template <int BLOCK_N, bool B_MN>
+static int launch_gemm_peer(const TmapArray& ta, const CUtensorMap& tb, const GemmParams& p, const PeerArgs& pa, int num_sms,
+                            cudaStream_t stream) {
+  using C = Cfg<BLOCK_N>;
+  auto kern = gemm_bf16_peer_kernel<BLOCK_N, B_MN>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
+    if (e != cudaSuccess) return (int)e;
+    configured = true;
+  }
+  int total = p.m_blocks * p.n_blocks * p.batch * p.split_k;
+  int grid = total < num_sms ? total : num_sms;
+  return (int)tepd::launch(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, ta, tb, p, pa);
+}
+
+// Tensor-parallel fused GEMMs over peer memory.
+//   mode 1 (GEMM -> reduce-scatter): A [M, K_local] local, B local; out_ptrs[r] = rank r's fp32 [M/n, N] buffer (pre-zeroed).
+//   mode 2 (all-gather -> GEMM)    : a_ptrs[r] = rank r's bf16 shard [M/n, K]; D local [M, N] (bf16 or fp32).
+//   mode 3 (GEMM -> reduce-scatter): as mode 1 but out_ptrs[r] = rank r's bf16 slot buffer [n, M/n, N]; follow with slot_reduce.
+//   mode 4 (all-gather -> GEMM)    : a_ptrs[rank] = own shard [M/n, K]; a_ptrs[(rank+1)%n] = local staging buffer [M, K] that
+//                                    p2p_gather_chunks fills; flags / epoch as published by that kernel.
+extern "C" int tepd_gemm_bf16_peer(int mode, void* const* a_ptrs, const void* B, void* D, void* const* out_ptrs, const void* bias,
+                                   int M, int N, int K, long long lda, long long ldb, long long ldd, int b_mn, int out_fp32,
+                                   int n_peers, int rank, int block_n, int num_sms, void* stream, const void* flags,
+                                   const void* epoch) {
+  if (N % 8 != 0 || K % 8 != 0 || n_peers < 1 || n_peers > MAX_PEERS || M % n_peers) return -2;
+  const int rows_per_owner = M / n_peers;
+  if (rows_per_owner % BLOCK_M) return -3;
+  GemmParams p;
+  p.M = M; p.N = N; p.K = K; p.batch = 1;
+  if (block_n != 128 && block_n != 256) block_n = (N % 256 == 0 || N > 1024) ? 256 : 128;
+  p.m_blocks = M / BLOCK_M;
+  p.n_blocks = (N + block_n - 1) / block_n;
+  p.k_blocks = (K + BLOCK_K - 1) / BLOCK_K;
+  p.split_k = 1; p.stream_k = 0; p.sk_ws = nullptr; p.sk_cnt = nullptr;
+  p.ldd = ldd; p.stride_d = 0; p.ld_res = 0; p.stride_res = 0;
+  const bool gather = mode == 2 || mode == 4;
+  p.D = D; p.bias = gather ? bias : nullptr; p.residual = nullptr; p.alpha = 1.0f;
+  p.out_fp32 = mode == 1 ? 1 : (mode == 3 ? 0 : out_fp32); p.accumulate = mode == 1 ? 1 : 0; p.act = 0; p.bias_bf16 = 0;
+  p.D2 = nullptr; p.aux = nullptr;
+  p.row_scale = nullptr; p.w_scale = nullptr; p.bias_stride = 0;
+  PeerArgs pa;
+  pa.mode = mode; pa.n = n_peers; pa.rank = rank; pa.rows_per_owner = rows_per_owner;
+  pa.flags = reinterpret_cast<const uint32_t*>(flags); pa.epoch = reinterpret_cast<const uint32_t*>(epoch);
+  if (mode == 4 && n_peers > 1 && (!flags || !epoch)) return -4;
+  for (int i = 0; i < MAX_PEERS; ++i) pa.out[i] = ((mode == 1 || mode == 3) && i < n_peers) ? out_ptrs[i] : nullptr;
+  TmapArray ta;
+  int rc;
+  for (int r = 0; r < n_peers; ++r) {
+    if (mode == 2)      rc = tepd_make_tmap_bf16_3d(&ta.m[r], a_ptrs[r], K, rows_per_owner, 1, lda, 0, BLOCK_K, BLOCK_M);
+    else if (mode == 4) rc = r == rank ? tepd_make_tmap_bf16_3d(&ta.m[r], a_ptrs[r], K, rows_per_owner, 1, lda, 0, BLOCK_K, BLOCK_M)
+                                       : tepd_make_tmap_bf16_3d(&ta.m[r], a_ptrs[(rank + 1) % n_peers], K, M, 1, lda, 0, BLOCK_K, BLOCK_M);
+    else                rc = tepd_make_tmap_bf16_3d(&ta.m[r], a_ptrs[0], K, M, 1, lda, 0, BLOCK_K, BLOCK_M);
+    if (rc) return 100 + rc;
+  }
+  for (int r = n_peers; r < MAX_PEERS; ++r) ta.m[r] = ta.m[0];
+  CUtensorMap tb;
+  if (!b_mn) rc = tepd_make_tmap_bf16_3d(&tb, B, K, N, 1, ldb, 0, BLOCK_K, block_n);
+  else       rc = tepd_make_tmap_bf16_3d(&tb, B, N, K, 1, ldb, 0, 64, BLOCK_K);
+  if (rc) return 200 + rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (num_sms <= 0) num_sms = tepd::num_sms();
+  if (block_n == 256) return b_mn ? launch_gemm_peer<256, true>(ta, tb, p, pa, num_sms, s) : launch_gemm_peer<256, false>(ta, tb, p, pa, num_sms, s);
+  return b_mn ? launch_gemm_peer<128, true>(ta, tb, p, pa, num_sms, s) : launch_gemm_peer<128, false>(ta, tb, p, pa, num_sms, s);
+}
+
+// ------------------------------------------------------------------ fp8 (e4m3) grouped GEMM for the MoE experts
+static int make_tmap_u8(CUtensorMap* out, const void* ptr, long long inner, long long rows, long long batch, int box_rows) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return -1;
+  cuuint64_t dims[3] = {(cuuint64_t)inner, (cuuint64_t)rows, (cuuint64_t)batch};
+  cuuint64_t strides[2] = {(cuuint64_t)inner, (cuuint64_t)(inner * rows)};
+  cuuint32_t box[3] = {128, (cuuint32_t)box_rows, 1}, es[3] = {1, 1, 1};
+  return fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS ? 0 : -2;
+}
+
+// D[b] (bf16 [M,N]) = act((A[b] (e4m3 [M,K]) . B[b]^T (e4m3 [N,K])) * row_scale[b,:] * w_scale[b] + bias[b])
+extern "C" int tepd_gemm_fp8(const void* A, const void* B, void* D, const void* row_scale, const void* w_scale, const void* bias, int M,
+                             int N, int K, int batch, int act, int num_sms, void* stream) {
+  if (K % 16 || N % 8 || M <= 0) return -2;
+  constexpr int BN = 128;
+  GemmParams p;
+  p.M = M; p.N = N; p.K = K; p.batch = batch;
+  p.m_blocks = (M + BLOCK_M - 1) / BLOCK_M; p.n_blocks = (N + BN - 1) / BN; p.k_blocks = (K + 127) / 128;
+  p.split_k = 1; p.stream_k = 0; p.sk_ws = nullptr; p.sk_cnt = nullptr;
+  p.ldd = N; p.stride_d = (long long)M * N; p.ld_res = 0; p.stride_res = 0;
+  p.D = D; p.bias = bias; p.residual = nullptr; p.alpha = 1.0f;
+  p.out_fp32 = 0; p.accumulate = 0; p.act = act == 1 ? 1 : 0; p.bias_bf16 = 0; p.D2 = nullptr; p.aux = nullptr;
+  p.row_scale = (const float*)row_scale; p.w_scale = (const float*)w_scale; p.bias_stride = N;
+  CUtensorMap ta, tb;
+  if (make_tmap_u8(&ta, A, K, M, batch, BLOCK_M) || make_tmap_u8(&tb, B, K, N, batch, BN)) return -3;
+  if (num_sms <= 0) num_sms = tepd::num_sms();
+  return launch_gemm<BN, false, false, true>(ta, tb, p, num_sms, reinterpret_cast<cudaStream_t>(stream));
+}

@@ -41,6 +41,8 @@ def plan_spmd(graph: Graph, num: int, strategy: str = "auto", options: Optional[
         o.mem_split_min_rank = 2
     from .. import config
     o.hw = config.hw_profile()
+    if strategy != "tp":
+        o.var_mem_limit = o.hw.var_mem_limit   # the profile's device budget unless VAR_MEM_LIMIT / options say otherwise
     config.check_num_gradients(sum(1 for n in graph.nodes if n.op.startswith("apply_")))
     for k, v in {**config.spmd_overrides(), **options}.items():   # flags (ServiceEnv) < explicit call arguments
         if hasattr(o, k):

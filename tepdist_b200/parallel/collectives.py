@@ -19,7 +19,7 @@ _REDUCE = {0: dist.ReduceOp.SUM, 1: dist.ReduceOp.MAX, 2: dist.ReduceOp.MIN, 3: 
 class CollectiveRunner:
     def __init__(self, mesh: DeviceMesh, comm_dtype: Optional[torch.dtype] = None):
         self.mesh = mesh
-        self.comm_dtype = comm_dtype  # FP16_COMM equivalent (bf16 on B200)
+        self.comm_dtype = comm_dtype  # FP16_COMM equivalent (bf16)
         self.bytes_moved = 0
         self.dry = False  # timing-only stand-ins (no communication), see Executor.dry_comm
 

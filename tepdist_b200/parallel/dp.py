@@ -2,7 +2,7 @@
 
 Baseline ("reference-semantics") mode issues NCCL all-reduces (the reference's DAPPLEAllReduceThunk,
 SURVEY K1, but bucketed as its unregistered DAPPLEAllReduceCombiner intended, B7).  The product path is the
-peer-memory reduce-scatter fused with scale (parallel/symm.py + ops/csrc/comm_sm100.cu).
+peer-memory reduce-scatter fused with scale (parallel/symm.py + ops/csrc/comm_sm90.cu).
 """
 from __future__ import annotations
 

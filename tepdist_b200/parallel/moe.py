@@ -1,7 +1,7 @@
-"""Fused expert-parallel MoE FFN forward over peer memory (kernels: ops/csrc/moe_sm100.cu).
+"""Fused expert-parallel MoE FFN forward over peer memory (kernels: ops/csrc/moe_sm90.cu).
 
     dispatch (quantise to e4m3 + P2P push into the expert owner's buffer)  ->  barrier
-    FC1 in fp8 on tcgen05 (per-token x per-expert scales, GELU fused)      ->  FC2 (bf16 tcgen05, batched over local experts)
+    FC1 in fp8 on wgmma (per-token x per-expert scales, GELU fused)      ->  FC2 (bf16 wgmma, batched over local experts)
     barrier  ->  combine (P2P pull of expert outputs, gate-weighted sum)
 
 Routing follows GShard local groups: every source rank owns `capacity` slots per expert, so slot assignment is a purely
@@ -97,7 +97,7 @@ class FusedMoE:
                                None if self.b1 is None else self.b1.data_ptr(), rows_per_e, self.H, M, self.El, 1, ops._sms(), s)
         assert rc == 0, rc
         y = self.y.tensor(torch.bfloat16, self.rows * M).view(self.El, rows_per_e, M)
-        ops.gemm(self.h, self.w2, out=y)          # FC2: batched bf16 tcgen05 GEMM over the local experts
+        ops.gemm(self.h, self.w2, out=y)          # FC2: batched bf16 wgmma GEMM over the local experts
         self.barrier()    # every expert output is in place
         out = torch.empty(T, M, dtype=torch.bfloat16, device=x.device)
         rc = lib.tepd_moe_combine(self.y.ptr_array, route.data_ptr(), gate.data_ptr(), out.data_ptr(), T, M, K, self.El, self.C, self.n,

@@ -1,4 +1,4 @@
-"""Symmetric (peer-mapped) device memory for the fused NVLink kernels (ops/csrc/comm_sm100.cu).
+"""Symmetric (peer-mapped) device memory for the fused NVLink kernels (ops/csrc/comm_sm90.cu).
 
 Every rank allocates the same-sized buffer, exports a CUDA IPC handle, and maps all peers' buffers; kernels then
 read / write peer memory directly over NVLink (P2P loads/stores), replacing NCCL for the hot collectives.
@@ -122,7 +122,7 @@ class SymmetricBuffer:
     backend 'vmm' (default on NVSwitch boxes): cuMemCreate physical pages, POSIX-fd handles exchanged over unix sockets,
     every peer's pages mapped into this process (`ptrs[r]`, unicast) AND all of them bound to one multicast object whose
     mapping `mc_ptr` addresses the n replicas at once: `multimem.ld_reduce` on it returns the switch-reduced value,
-    `multimem.st` writes every replica (ops/csrc/vmm_sm100.cu).  backend 'ipc': cudaMalloc + cudaIpc handles, `mc_ptr` None."""
+    `multimem.st` writes every replica (ops/csrc/vmm_sm90.cu).  backend 'ipc': cudaMalloc + cudaIpc handles, `mc_ptr` None."""
 
     def __init__(self, nbytes: int, group=None, backend: Optional[str] = None):
         self.lib = ops.lib()
@@ -319,10 +319,8 @@ class FusedShardedOptimizer:
     Multicast-bound buffers (backend 'vmm'): the NVLS kernel -- the gradient chunk arrives already summed by the switch
     (`multimem.ld_reduce`, one load per 16 bytes instead of n-1 peer loads) and the updated bf16 shard leaves the GPU once
     (`multimem.st`, replicated by the switch instead of n-1 peer stores); barriers are one `multimem.red` per rank with a
-    bounded spin.  Opt-in (TEPDIST_DP_MC=1): measured on 4 x B200 the fp32 switch reduction is SLOWER than unicast peer loads for
-    this kernel (8M parameters: 122 us vs 74 us; GPT-2 345M dp4 step 20.1 vs 17.5 ms) -- a reduce-scatter through the switch
-    still costs every GPU its full gradient buffer in egress, so NVLS only pays for the all-gather half; with a bf16 gradient
-    wire it is 55 us.  Default: unicast P2P loads / stores (IPC or VMM mappings alike)."""
+    bounded spin.  Opt-in (TEPDIST_DP_MC=1): a reduce-scatter through the switch still costs every GPU its full gradient buffer
+    in egress, so NVLS only pays for the all-gather half.  Default: unicast P2P loads / stores (IPC or VMM mappings alike)."""
 
     def __init__(self, grad_buf: SymmetricBuffer, param_buf: SymmetricBuffer, group=None, grad16_buf: Optional[SymmetricBuffer] = None):
         import os
@@ -423,7 +421,7 @@ def all_gather_gemm(x_shard: SymmetricBuffer, rows_per_rank: int, K: int, w: tor
 
 class GemmReduceScatter:
     """Row-parallel linear + reduce-scatter without atomics on the wire: the GEMM epilogue writes each bf16 partial row
-    block into slot [my rank] of the OWNER's staging buffer with plain 16-byte NVLink stores (gemm_sm100.cu peer mode 3),
+    block into slot [my rank] of the OWNER's staging buffer with plain 16-byte NVLink stores (gemm_sm90.cu peer mode 3),
     one flag barrier later the owner sums its n slots (+ bias + residual) in a single pass (slot_reduce).  Two staging
     buffers alternate so the barrier that publishes round i also protects the slots of round i-1 from being overwritten
     early.  Replaces the reference's dot -> in-stream NCCL all-reduce pair (SURVEY 2.H K1; service/gpu/
@@ -519,7 +517,7 @@ class GemmAllReduce:
 
 
 class GemmAllReduceMC:
-    """Row-parallel linear + ALL-reduce over NVLS: the tcgen05 GEMM writes its bf16 partial [M, N] straight into a
+    """Row-parallel linear + ALL-reduce over NVLS: the wgmma GEMM writes its bf16 partial [M, N] straight into a
     symmetric buffer (no staging copy), then ONE multimem kernel reduces it inside the NVSwitch -- every rank pulls its 1/n
     slice with `multimem.ld_reduce` (fp32 accumulation in the switch), adds bias + residual and publishes the finished
     rows to all ranks with `multimem.st`; the two cross-rank barriers live inside that kernel (one `multimem.red` per CTA).

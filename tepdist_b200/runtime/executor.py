@@ -1,10 +1,10 @@
 """Graph executor: runs one (sub-)graph of planner IR on one device.
 
-Design (B200-first, replaces XLA executables + thunk sequences of the reference — SURVEY §3.3/3.4):
+Design (H100-first, replaces XLA executables + thunk sequences of the reference — SURVEY §3.3/3.4):
   * variables live on the device across steps in FLAT buffers (fp32 master, bf16 compute copy, fp32
     gradient accumulators, optimizer slots) so the optimizer update, gradient zeroing ("GAInit") and
     the data-parallel gradient reduction are each ONE kernel / collective over contiguous memory;
-  * every node maps onto a hand-written sm_100a kernel (tepdist_b200.ops) on the hot path;
+  * every node maps onto a hand-written sm_90a kernel (tepdist_b200.ops) on the hot path;
   * activations are freed by a liveness plan computed once (the reference's
     OutputBuffersLifeTimeTracker / MakeTaskGraphGCPlan, SURVEY D5/D6);
   * the whole step is captured into a CUDA graph after warm-up, so the host-side interpreter cost
@@ -25,8 +25,8 @@ from ..utils.init import init_tensor
 
 # tensor-parallel plans: run `linear -> all_reduce [-> + bias] [-> + residual]` as GEMM -> all-reduce over peer memory
 # (parallel/symm.py GemmAllReduceMC: GEMM into a multicast-bound buffer + ONE multimem reduction kernel with bias / residual
-# fused) instead of GEMM + NCCL + separate adds.  Default in comm = "fused" mode (validated on 2 / 4 / 8 B200: 1.10x / 1.25x /
-# 1.51x the NCCL arm of the same plan, profiles/round2); TEPDIST_TP_FUSED=0 or comm = "nccl" selects the library collectives.
+# fused) instead of GEMM + NCCL + separate adds.  Default in comm = "fused" mode; TEPDIST_TP_FUSED=0 or comm = "nccl" selects
+# the library collectives.
 TP_FUSED = os.environ.get("TEPDIST_TP_FUSED", "1") == "1"
 # test hook: a factory (M, N, group, barrier) -> object with new_output() / __call__(x, w, out, bias, residual, b_mn) that
 # stands in for parallel.symm.GemmAllReduce, so the executor-side chain fusion can be exercised on CPU (gloo) where the
@@ -345,7 +345,7 @@ class Executor:
                     last_use[o.key()] = max(last_use.get(o.key(), 0), p_.id)
                     break
         # peephole: gelu(linear(x)) -> one GEMM writing pre-activation + activation; gelu_bwd(linear_dgrad(dz), f) ->
-        # the dgrad GEMM multiplies by GELU'(f) in its epilogue (GPU only: these are epilogues of the tcgen05 kernel)
+        # the dgrad GEMM multiplies by GELU'(f) in its epilogue (GPU only: these are epilogues of the wgmma kernel)
         self.gelu_dual: Dict[int, int] = {}
         self.gelu_bwd_fuse: Dict[int, Tuple[int, int]] = {}
         if self.device.type == "cuda":
@@ -560,7 +560,7 @@ class Executor:
                 fo.barrier()
                 fo.step(st.master, st.m, st.v, s0 + r * chunk, s0 + (r + 1) * chunk, st.n_decay, self.hyper,
                         o.get("beta1", 0.9), o.get("beta2", 0.999), o.get("eps", 1e-8), o.get("weight_decay", 0.0),
-                        ctas=0 if last else int(os.environ.get("TEPDIST_OVERLAP_CTAS", o.get("overlap_ctas", 74))))   # 74: measured A/B on 4 x B200, 16.89 vs 17.37 ms with 296 (37: 17.88)
+                        ctas=0 if last else int(os.environ.get("TEPDIST_OVERLAP_CTAS", o.get("overlap_ctas", ops._sms() // 2))))   # half the SMs; the rest stay with the backward kernels
             pending.append(None)
             return
         s0, e0 = fz["buckets"][bi]
@@ -1603,13 +1603,13 @@ class Executor:
                 dense.scatter_(2, flat, dots)
                 return [dense[:, :, :rt["E"] * rt["C"]].reshape(Gn, Sn, rt["E"], rt["C"]).to(torch_dtype(n.outputs[0].dtype, self.device))]
         if op == "einsum":
-            # own batched tcgen05 GEMM for bf16 operands on the GPU (expert FFNs, dispatch / combine and their gradients);
+            # own batched wgmma GEMM for bf16 operands on the GPU (expert FFNs, dispatch / combine and their gradients);
             # torch.einsum for the CPU oracle and for patterns outside the kernel's alignment rules
             if (ins[0].is_cuda and ins[0].dtype == torch.bfloat16 and ins[1].dtype == torch.bfloat16
                     and os.environ.get("TEPDIST_EINSUM", "own") != "torch"):
                 return [ops.einsum(a["eq"], ins[0], ins[1])]
             return [torch.einsum(a["eq"], ins[0], ins[1])]
-        # convolutions: own path = NHWC im2col / col2im kernels + tcgen05 GEMMs (ops/csrc/conv_sm100.cu); cuDNN through torch
+        # convolutions: own path = NHWC im2col / col2im kernels + wgmma GEMMs (ops/csrc/conv_sm90.cu); cuDNN through torch
         # is the reference-semantics path (TEPDIST_CONV=cudnn) and the CPU oracle
         if op == "conv2d":
             if ops.conv_native_ok(ins[0], ins[1]):
@@ -1656,7 +1656,7 @@ class Executor:
             dg = self._grad_out(n, 1, n.outputs[1].shape); dg.add_((dyf * xh).sum((0, 2, 3)))
             db = self._grad_out(n, 2, n.outputs[2].shape); db.add_(dyf.sum((0, 2, 3)))
             return [dx.to(xx.dtype), dg, db]
-        # pooling: own NHWC kernels on the GPU (conv_sm100.cu; gather-form max-pool backward from the saved input / output instead of
+        # pooling: own NHWC kernels on the GPU (conv_sm90.cu; gather-form max-pool backward from the saved input / output instead of
         # re-running the forward under autograd), torch ops on CPU
         if op == "maxpool2d": return [ops.maxpool2d_fwd(x, a["k"], a["stride"], a["padding"])]
         if op == "maxpool2d_bwd": return [ops.maxpool2d_bwd(ins[0], ins[1], ins[2], a["k"], a["stride"], a["padding"])]

@@ -22,7 +22,7 @@ def case_gpt2(strategy, feed_shards=False, batch=4):
     cfg = CONFIGS["tiny"]
     if strategy.startswith(("pp", "cp", "dp2cp")) and int(os.environ.get("WORLD_SIZE", "1")) == 1:
         strategy = "auto"   # single-process oracle
-    if os.environ.get("TEPDIST_TEST_NCTX"):     # (GPU runs of the ring: blocks of 128 tokens go through the tcgen05 kernels)
+    if os.environ.get("TEPDIST_TEST_NCTX"):     # (GPU runs of the ring: blocks of 128 tokens go through the wgmma kernels)
         import dataclasses
         cfg = dataclasses.replace(cfg, n_ctx=int(os.environ["TEPDIST_TEST_NCTX"]))
     g = build_gpt2_graph(cfg, batch=batch)

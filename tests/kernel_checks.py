@@ -1,4 +1,4 @@
-"""Numerics + timing checks for the sm_100a kernels against plain-PyTorch fp32 references.
+"""Numerics + timing checks for the sm_90a kernels against plain-PyTorch fp32 references.
 
 Used two ways: (1) `python tests/kernel_checks.py [names...]` on a GPU box runs every check in its own
 subprocess with a timeout (so one hung kernel cannot take the whole run down) and writes
@@ -153,7 +153,8 @@ def check_gemm_epilogues():
 
 
 def check_gemm2():
-    """2-CTA (cta_group::2) kernel: numerics vs fp32 reference for both B layouts + fused epilogues, then throughput."""
+    """ops.gemm2 (128x256 tiles, explicit tile-parallel / stream-K schedule): numerics vs fp32 reference for both B layouts +
+    fused epilogues, then throughput."""
     from tepdist_b200 import ops
     out = {}
     torch.manual_seed(7)
@@ -258,7 +259,7 @@ def check_gemm_perf():
     out["ours_wgrad_4096tok_1024x4096_tflops"] = 2.0 * T * N * K / ms / 1e9
     ms = _time_ms(lambda: torch.matmul(dY.t(), X))
     out["cublas_wgrad_tflops"] = 2.0 * T * N * K / ms / 1e9
-    # stream-K + fix-up vs the tile-parallel 1-CTA / 2-CTA kernels and cuBLAS on the forward and dgrad shapes
+    # stream-K + fix-up vs the tile-parallel schedules (128- and 256-wide tiles) and cuBLAS on the forward and dgrad shapes
     for (M, N, K, bmn) in [(4096, 3072, 1024, False), (4096, 1024, 1024, False), (4096, 4096, 1024, False), (4096, 1024, 4096, False),
                            (4096, 1024, 3072, True), (4096, 1024, 4096, True), (4096, 4096, 1024, True)]:
         A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
@@ -272,8 +273,8 @@ def check_gemm_perf():
         out[f"cta2_{tag}_tflops"] = 2.0 * M * N * K / ms / 1e9
         ms = _time_ms(lambda: torch.matmul(A, W if bmn else W.t()))
         out[f"cublas_{tag}_tflops"] = 2.0 * M * N * K / ms / 1e9
-    # wave-quantisation probe: 37 m-blocks x {4, 16} n-blocks = exact multiples of 148 tiles vs the 32 m-block shapes
-    for (M, N, K) in [(4736, 1024, 4096), (4736, 4096, 1024), (4736, 3072, 1024)]:
+    # wave-quantisation probe: 33 m-blocks x {4, 16} n-blocks = exact multiples of 132 tiles vs the 32 m-block shapes
+    for (M, N, K) in [(4224, 1024, 4096), (4224, 4096, 1024), (4224, 3072, 1024)]:
         A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
         W = torch.randn(N, K, device="cuda", dtype=torch.bfloat16)
         ms = _time_ms(lambda: ops.gemm(A, W, block_n=256))
@@ -302,7 +303,7 @@ def check_gemm_perf():
 
 
 def check_conv():
-    """NHWC im2col / col2im kernels + tcgen05 GEMMs vs torch (cuDNN) convolutions in fp32 on the same bf16 inputs."""
+    """NHWC im2col / col2im kernels + wgmma GEMMs vs torch (cuDNN) convolutions in fp32 on the same bf16 inputs."""
     import torch.nn.functional as F
     from tepdist_b200 import ops
     out = {}
@@ -501,30 +502,6 @@ def check_attn_d48():
     return out
 
 
-def check_attn_poly():
-    """POLY instantiations (every second exponential on the FMA pipes, TEPDIST_ATTN_EXP_POLY=1): same numerics checks as the
-    default kernels + timing.  Run as its own process (the switch is read once): python tests/kernel_checks.py attn_poly"""
-    os.environ["TEPDIST_ATTN_EXP_POLY"] = "1"
-    out = {"fwd": check_attn_fwd(), "bwd": check_attn_bwd()}
-    try:
-        out["perf"] = check_attn_perf()
-    except Exception as e:  # noqa: BLE001
-        out["perf"] = repr(e)
-    return out
-
-
-def check_attn_fwd2():
-    """Experimental two-query-tile forward (TEPDIST_ATTN_FWD2=1): numerics of check_attn_fwd on the S % 256 == 0 cases +
-    timing.  Own process: python tests/kernel_checks.py attn_fwd2"""
-    os.environ["TEPDIST_ATTN_FWD2"] = "1"
-    out = {"fwd": check_attn_fwd()}
-    try:
-        out["perf"] = check_attn_perf()
-    except Exception as e:  # noqa: BLE001
-        out["perf"] = repr(e)
-    return out
-
-
 def check_attn_bwd():
     from tepdist_b200 import ops
     from tepdist_b200.ops.attention import _ref_fwd
@@ -575,7 +552,7 @@ def check_attn_perf():
 
 
 def check_einsum():
-    """ops.einsum (one batched tcgen05 GEMM per einsum) on the GPT-MoE patterns: forward and gradient equations, both operand
+    """ops.einsum (one batched wgmma GEMM per einsum) on the GPT-MoE patterns: forward and gradient equations, both operand
     majors, with and without the layout copies; vs torch.einsum in fp32.  Then throughput of the expert FC vs torch.einsum."""
     from tepdist_b200 import ops
     out = {}
@@ -588,7 +565,7 @@ def check_einsum():
         ia, ib = eq.split("->")[0].split(",")
         n0 = ops.launch_count()
         got = ops.einsum(eq, t[ia], t[ib])
-        assert ops.launch_count() > n0, eq           # the tcgen05 GEMM ran, not the torch fallback
+        assert ops.launch_count() > n0, eq           # the wgmma GEMM ran, not the torch fallback
         ref = torch.einsum(eq, t[ia].float(), t[ib].float())
         out[eq] = _rel_err(got, ref)
         assert out[eq] < 1e-2, (eq, out[eq])
@@ -777,8 +754,6 @@ CHECKS = {
     "moe_routes": check_moe_routes,
     "ew": check_ew,
     "attn_d48": check_attn_d48,
-    "attn_poly": check_attn_poly,
-    "attn_fwd2": check_attn_fwd2,
     "gemm2": check_gemm2,
     "attn_perf": check_attn_perf,
 }

@@ -1,4 +1,4 @@
-"""2+ GPU worker: NVLS substrate (VMM allocation + multicast binding) and the multimem kernels of ops/csrc/vmm_sm100.cu
+"""2+ GPU worker: NVLS substrate (VMM allocation + multicast binding) and the multimem kernels of ops/csrc/vmm_sm90.cu
 against plain references, plus timing against NCCL.  Writes a JSON report; prints one line per stage so a failure is
 attributable from the log alone."""
 import json

@@ -1,4 +1,4 @@
-"""2+ GPU worker: fused expert-parallel MoE forward (fp8 dispatch + tcgen05 fp8 FC) vs a dense fp32 reference."""
+"""2+ GPU worker: fused expert-parallel MoE forward (fp8 dispatch + wgmma fp8 FC) vs a dense fp32 reference."""
 import json
 import os
 import sys

@@ -1,4 +1,4 @@
-"""GPU numerics: every sm_100a kernel vs a plain PyTorch fp32 reference (see tests/kernel_checks.py)."""
+"""GPU numerics: every sm_90a kernel vs a plain PyTorch fp32 reference (see tests/kernel_checks.py)."""
 import pytest
 import torch
 

@@ -66,7 +66,7 @@ def test_pipeline_x_spmd_and_2d_mesh_on_four_gpus_match_one_gpu(tmp_path):
 def test_context_parallel_ring_attention_on_two_gpus_matches_one_gpu(tmp_path):
     """`cp`: the sequence (256 tokens) is cut in two blocks of 128, every token-wise op runs on its block, attention keeps its
     queries and passes K / V (forward) and K / V + the fp32 dK / dV accumulators (backward) around the ring over NCCL; the
-    diagonal block runs the causal tcgen05 kernel, the off-diagonal one the unmasked kernel, partial outputs merge by
+    diagonal block runs the causal attention kernel, the off-diagonal one the unmasked kernel, partial outputs merge by
     log-sum-exp (parallel/ring_attention.py)."""
     env = {"TEPDIST_TEST_NCTX": "256"}
     ref = _run("gpt2:auto", 1, tmp_path, env)
@@ -78,7 +78,7 @@ def test_context_parallel_ring_attention_on_two_gpus_matches_one_gpu(tmp_path):
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_context_parallel_zigzag_on_two_gpus_matches_one_gpu(tmp_path):
     """Load-balanced (zig-zag) ring: 512 tokens = 4 chunks of 128; rank 0 computes for chunks (0, 3), rank 1 for (1, 2); the
-    half-block products run the same tcgen05 block kernels as the contiguous ring."""
+    half-block products run the same attention block kernels as the contiguous ring."""
     env = {"TEPDIST_TEST_NCTX": "512", "TEPDIST_CP_ZIGZAG": "1"}
     ref = _run("gpt2:auto", 1, tmp_path, env)
     got = _run("gpt2:cp", 2, tmp_path, env)
