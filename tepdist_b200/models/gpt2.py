@@ -48,6 +48,9 @@ CONFIGS = {
     "PrettyBig": GPT2Config(25, 1024, 16, 1024, 50257, 4, lr=2.5e-4, name="gpt2-PrettyBig"),
     "175B": GPT2Config(96, 12288, 96, 12288, 50257, 4, lr=2.5e-4, name="gpt2-175B"),
     "tiny": GPT2Config(2, 128, 2, 128, 1000, 2, name="gpt2-tiny"),
+    # GPT-3 XL shape (Brown et al. 2020, Table 2.1): 16 heads of 128
+    "1.3B": GPT2Config(24, 2048, 16, 2048, 50257, 4, name="gpt3-xl-1.3B"),
+    "tiny-hd128": GPT2Config(2, 256, 2, 128, 1000, 2, name="gpt2-tiny-hd128"),
 }
 
 

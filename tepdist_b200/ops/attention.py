@@ -3,6 +3,10 @@
 Tensors use the "bshd" convention: q/k/v are views [B, S, H, D] (arbitrary batch/seq/head strides, D
 contiguous) — typically slices of the fused qkv projection output [B, S, H, 3, D] (heads-major); the output is a
 contiguous [B, S, H, D] tensor, i.e. already the [tokens, hidden] input of the output projection.
+
+On CUDA tensors the wgmma kernels cover head widths 64 and 128 with S % 128 == 0; narrower heads and a ragged causal
+sequence length are zero-padded onto them (see `_can_pad`).  The remaining shapes (D > 128, non-causal ragged S) run
+plain torch math, which materialises [B, H, S, S] fp32 scores, and warn once per shape.
 """
 from __future__ import annotations
 
@@ -10,21 +14,33 @@ import math
 
 import torch
 
-_HD = 64   # head dim of the wgmma kernels (attention_sm90.cu)
+_KERNEL_WIDTHS = (64, 128)   # head dims of the wgmma kernels (attention_sm90.cu)
+
+
+def _kernel_width(D: int) -> int | None:
+    """The kernel head width a D-wide head runs on (zero-padded up to it), or None when no kernel is wide enough."""
+    return next((w for w in _KERNEL_WIDTHS if D <= w), None)
 
 
 def _can_pad(S: int, D: int, causal: bool) -> bool:
-    """Shapes that run on the D = 64 / S % 128 == 0 kernels through zero padding, exactly:
-       * narrower heads: padded q.k terms are zero, padded V / O columns are dropped;
+    """Shapes that run on the D = 64 / 128, S % 128 == 0 kernels through zero padding, exactly:
+       * narrower heads (D <= 64 -> 64, 64 < D <= 128 -> 128): padded q.k terms are zero, padded V / O columns are
+         dropped;
        * a ragged sequence length under a CAUSAL mask: padded keys sit after every real query (masked), padded query rows
          are dropped, and their zero dO makes their contribution to dK / dV vanish."""
-    return D <= _HD and (S % 128 == 0 or causal)
+    return _kernel_width(D) is not None and (S % 128 == 0 or causal)
 
 
-def _pad_sd(t: torch.Tensor, S: int, D: int) -> torch.Tensor:
-    """[B, S, H, D] -> zero-padded contiguous [B, ceil128(S), H, 64]."""
+def _pad_sd(t: torch.Tensor, S: int, D: int, W: int) -> torch.Tensor:
+    """[B, S, H, D] -> zero-padded contiguous [B, ceil128(S), H, W]."""
     Sp = (S + 127) // 128 * 128
-    return torch.nn.functional.pad(t, (0, _HD - D, 0, 0, 0, Sp - S))
+    return torch.nn.functional.pad(t, (0, W - D, 0, 0, 0, Sp - S))
+
+
+def _warn_torch_math(S: int, D: int, causal: bool) -> None:
+    from . import _warn_once
+    _warn_once(f"attention: no kernel for head dim {D}, seq {S}, causal={causal}; running torch math with "
+               f"[B, H, {S}, {S}] fp32 scores")
 
 
 def _ref_fwd(q, k, v, scale, causal):
@@ -50,12 +66,14 @@ def attention_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: floa
     if not q.is_cuda:
         o, lse, _ = _ref_fwd(q, k, v, scale, causal)
         return o, lse
-    if D != _HD or S % 128:
+    if D not in _KERNEL_WIDTHS or S % 128:
         if _can_pad(S, D, causal):
-            qp, kp, vp = (_pad_sd(t, S, D) for t in (q, k, v))
+            W = _kernel_width(D)
+            qp, kp, vp = (_pad_sd(t, S, D, W) for t in (q, k, v))
             o, lse = attention_fwd(qp, kp, vp, scale, causal)
             return o[:, :S, :, :D].contiguous(), lse[:, :, :S].contiguous()
-        o, lse, _ = _ref_fwd(q, k, v, scale, causal)   # shapes the wgmma kernel does not cover: plain torch math
+        _warn_torch_math(S, D, causal)
+        o, lse, _ = _ref_fwd(q, k, v, scale, causal)   # shapes the wgmma kernels do not cover: plain torch math
         return o, lse
     from . import lib, _check, _count, _stream
     assert q.dtype == torch.bfloat16 and q.stride(3) == 1
@@ -78,14 +96,16 @@ def attention_bwd(do: torch.Tensor, q, k, v, o, lse, scale: float | None = None,
     if dqkv_out is None:
         dqkv_out = torch.empty(B, S, H, 3, D, dtype=q.dtype, device=q.device)
     dq, dk, dv = dqkv_out[:, :, :, 0], dqkv_out[:, :, :, 1], dqkv_out[:, :, :, 2]
-    if q.is_cuda and (D != _HD or S % 128) and _can_pad(S, D, causal):
+    if q.is_cuda and (D not in _KERNEL_WIDTHS or S % 128) and _can_pad(S, D, causal):
         Sp = (S + 127) // 128 * 128
+        W = _kernel_width(D)
         lse_p = lse if Sp == S else torch.nn.functional.pad(lse, (0, Sp - S))
-        gq, gk, gv = attention_bwd(_pad_sd(do, S, D), _pad_sd(q, S, D), _pad_sd(k, S, D), _pad_sd(v, S, D), _pad_sd(o, S, D),
-                                   lse_p, scale, causal)
+        gq, gk, gv = attention_bwd(*(_pad_sd(t, S, D, W) for t in (do, q, k, v, o)), lse_p, scale, causal)
         dq.copy_(gq[:, :S, :, :D]); dk.copy_(gk[:, :S, :, :D]); dv.copy_(gv[:, :S, :, :D])
         return dq, dk, dv
-    if not q.is_cuda or D != _HD or S % 128:
+    if not q.is_cuda or D not in _KERNEL_WIDTHS or S % 128:
+        if q.is_cuda:
+            _warn_torch_math(S, D, causal)
         dof = do.float().permute(0, 2, 1, 3)
         qf, kf, vf = (t.float().permute(0, 2, 1, 3) for t in (q, k, v))
         # probabilities from the GIVEN log-sum-exp (like the kernels): a block of a longer key sequence (ring attention) passes

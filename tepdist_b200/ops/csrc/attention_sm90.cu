@@ -1,11 +1,14 @@
-// Fused (flash) attention for sm_90a, head_dim 64, bf16, with wgmma.mma_async on register accumulators.
-// Forward, one CTA per (128-query block, batch, head): two warpgroups own 64 query rows each, a producer warp streams K / V
-// tiles through a TMA + mbarrier ring.
+// Fused (flash) attention for sm_90a, head_dim 64 or 128, bf16, with wgmma.mma_async on register accumulators.
+// Forward, one CTA per (128-query block, batch, head): two warpgroups own 64 query rows each, a producer (one warp at
+// D = 64, a warpgroup at D = 128) streams K / V tiles through a TMA + mbarrier ring.
 //   S = Q K^T            wgmma m64n128k16 (A = Q, B = K, both K-major in smem)        -> registers
 //   P = online softmax   in registers (quad shuffles for the row max / sum)
-//   O += P V             wgmma m64n64k16 with A = P from registers (the S fragment repacked to bf16), B = V MN-major
+//   O += P V             wgmma m64nDk16 with A = P from registers (the S fragment repacked to bf16), B = V MN-major
 // Q/K/V are read straight out of the fused qkv projection buffer [B, S, H, 3, D] (heads-major) with 4-D TMA maps
 // (no head-split transposes), O is written as [B, S, H, D] so it feeds the output projection GEMM.
+// A D-wide row tile is D / 64 SW128 column chunks of [rows x 64] (128 B per row), each loaded by one TMA box.
+// At D = 128 the O (fwd) and dK + dV (bwd) accumulators double: the producer warpgroup drops to 24 registers with
+// setmaxnreg and the two consumer warpgroups take 240 each, so neither kernel spills.
 // The reference gets attention from XLA-fused batched dots + softmax fusions (SURVEY Appendix C);
 // this kernel is the H100-native replacement.
 #include "sm90_ptx.cuh"
@@ -17,18 +20,34 @@ using namespace sm90;
 
 namespace {
 
-constexpr int HD = 64;        // head dim
 constexpr int BQ = 128;       // query rows per forward CTA
 constexpr int BKV = 128;      // kv rows per forward iteration / per backward CTA
-constexpr int KV_STAGES = 3;
-constexpr int THREADS = 288;  // warps 0..7: two compute warpgroups, warp 8: TMA producer
+constexpr int CHUNK = 128 * 128;  // 16 KB: one [128 x 64] bf16 SW128 column chunk of a 128-row tile
 
-constexpr int TILE_BYTES = 128 * HD * 2;  // 16 KB: a [128 x 64] bf16 tile (one SW128 chunk)
-constexpr int SM_Q = 0;
-constexpr int SM_K = SM_Q + TILE_BYTES;
-constexpr int SM_V = SM_K + KV_STAGES * TILE_BYTES;
-constexpr int SM_BAR = SM_V + KV_STAGES * TILE_BYTES;
-constexpr int FWD_SMEM = SM_BAR + 256 + 1024;
+template <int HD>
+struct AttnCfg;
+template <>
+struct AttnCfg<64> {
+  static constexpr int THREADS = 288;  // warps 0..7: two compute warpgroups, warp 8: TMA producer
+  static constexpr int KV_STAGES = 3;
+  static constexpr int Q_STAGES = 3;
+};
+template <>
+struct AttnCfg<128> {
+  static constexpr int THREADS = 384;  // warpgroups 0, 1: compute (240 registers), warpgroup 2: TMA producer (24)
+  static constexpr int KV_STAGES = 2;  // 32 KB Q + 2 x 64 KB K / V
+  static constexpr int Q_STAGES = 3;   // 64 KB K / V + 16 KB dS^T + 3 x 32 KB Q / dO
+};
+
+template <int HD>
+struct FwdSmem {
+  static constexpr int TILE_BYTES = 128 * HD * 2;  // a [128 x HD] bf16 tile (HD / 64 chunks)
+  static constexpr int SM_Q = 0;
+  static constexpr int SM_K = SM_Q + TILE_BYTES;
+  static constexpr int SM_V = SM_K + AttnCfg<HD>::KV_STAGES * TILE_BYTES;
+  static constexpr int SM_BAR = SM_V + AttnCfg<HD>::KV_STAGES * TILE_BYTES;
+  static constexpr int BYTES = SM_BAR + 256 + 1024;
+};
 
 struct AttnFwdParams {
   void* O;      // bf16 [B, S, H, D]
@@ -42,12 +61,16 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-__global__ void __launch_bounds__(THREADS, 1)
+template <int HD>
+__global__ void __launch_bounds__(AttnCfg<HD>::THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const AttnFwdParams p) {
+  using L = FwdSmem<HD>;
+  constexpr int KV_STAGES = AttnCfg<HD>::KV_STAGES;
+  constexpr int NC = HD / 64;   // column chunks per row tile
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SM_BAR);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::SM_BAR);
   uint64_t* q_full = bars;
   uint64_t* kv_full = bars + 1;               // [KV_STAGES]
   uint64_t* kv_empty = bars + 1 + KV_STAGES;  // [KV_STAGES]
@@ -74,41 +97,48 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   __syncthreads();
   pdl_wait();
 
-  if (warp == 8) {
-    if (lane == 0) {
-      mbar_expect_tx(q_full, TILE_BYTES);
-      tma_load_4d(smem + SM_Q, &tmap_q, q_full, 0, qi * BQ, h, b);
+  if (HD == 64 ? warp == 8 : warp >= 8) {   // producer: warp 8 (D = 64) / warpgroup 2 (D = 128)
+    if constexpr (HD == 128) setmaxnreg_dec<24>();
+    if (lane == 0 && (HD == 64 || warp == 8)) {
+      mbar_expect_tx(q_full, L::TILE_BYTES);
+#pragma unroll
+      for (int c = 0; c < NC; ++c) tma_load_4d(smem + L::SM_Q + c * CHUNK, &tmap_q, q_full, c * 64, qi * BQ, h, b);
       for (int j = 0; j < nkv; ++j) {
         const int st = j % KV_STAGES;
         mbar_wait(&kv_empty[st], ((j / KV_STAGES) & 1) ^ 1);
-        mbar_expect_tx(&kv_full[st], 2 * TILE_BYTES);
-        tma_load_4d(smem + SM_K + st * TILE_BYTES, &tmap_k, &kv_full[st], 0, j * BKV, h, b);
-        tma_load_4d(smem + SM_V + st * TILE_BYTES, &tmap_v, &kv_full[st], 0, j * BKV, h, b);
+        mbar_expect_tx(&kv_full[st], 2 * L::TILE_BYTES);
+#pragma unroll
+        for (int c = 0; c < NC; ++c)
+          tma_load_4d(smem + L::SM_K + st * L::TILE_BYTES + c * CHUNK, &tmap_k, &kv_full[st], c * 64, j * BKV, h, b);
+#pragma unroll
+        for (int c = 0; c < NC; ++c)
+          tma_load_4d(smem + L::SM_V + st * L::TILE_BYTES + c * CHUNK, &tmap_v, &kv_full[st], c * 64, j * BKV, h, b);
       }
     }
     pdl_trigger();
     return;
   }
+  if constexpr (HD == 128) setmaxnreg_inc<240>();
 
   const int wg = warp >> 2;
   const int g = lane >> 2, q = lane & 3;
   const int row0 = wg * 64 + (warp & 3) * 16 + g;   // query row (in the tile) of fragment rows e < 2; +8 for e >= 2
-  const uint32_t sq = smem_u32(smem + SM_Q) + wg * 64 * 128;
-  float o[32];
+  const uint32_t sq = smem_u32(smem + L::SM_Q) + wg * 64 * 128;
+  float o[HD / 2];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   mbar_wait(q_full, 0);
   for (int j = 0; j < nkv; ++j) {
     const int st = j % KV_STAGES;
     mbar_wait(&kv_full[st], (j / KV_STAGES) & 1);
-    const uint32_t sk = smem_u32(smem + SM_K + st * TILE_BYTES), sv = smem_u32(smem + SM_V + st * TILE_BYTES);
+    const uint32_t sk = smem_u32(smem + L::SM_K + st * L::TILE_BYTES), sv = smem_u32(smem + L::SM_V + st * L::TILE_BYTES);
     float s[64];
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
-      wgmma_m64n128k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sq + k * 32, 0, 1024), make_smem_desc_sw128(sk + k * 32, 0, 1024),
-                                     k > 0 ? 1u : 0u);
+    for (int k = 0; k < HD / 16; ++k)
+      wgmma_m64n128k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sq + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024),
+                                     make_smem_desc_sw128(sk + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024), k > 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(s);
@@ -145,7 +175,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       }
       l[hr] = l[hr] * alpha + sum;
 #pragma unroll
-      for (int jj = 0; jj < 8; ++jj) {
+      for (int jj = 0; jj < HD / 8; ++jj) {
         o[4 * jj + 2 * hr] *= alpha;
         o[4 * jj + 2 * hr + 1] *= alpha;
       }
@@ -155,7 +185,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     for (int kk = 0; kk < 8; ++kk) {
       uint32_t a[4];
       frag_a_from_acc(s, kk, a);
-      wgmma_m64n64k16_bf16_rs<1>(o, a, make_smem_desc_sw128(sv + kk * 16 * 128, 8192, 1024), 1u);
+      // V MN-major: LBO = the next 64-column chunk (the field is unused at N = 64)
+      wgmma_m64nXk16_bf16_rs<1>(o, a, make_smem_desc_sw128(sv + kk * 16 * 128, HD == 64 ? 8192 : CHUNK, 1024), 1u);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -172,7 +203,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     const int row = qi * BQ + row0 + hr * 8;
     __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.O) + (((size_t)b * p.S + row) * p.H + h) * HD;
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj)
+    for (int jj = 0; jj < HD / 8; ++jj)
       *reinterpret_cast<uint32_t*>(op + 8 * jj + 2 * q) = pack_bf16x2(o[4 * jj + 2 * hr] * inv, o[4 * jj + 2 * hr + 1] * inv);
     if (q == 0) p.lse[((size_t)b * p.H + h) * p.S + row] = (m[hr] + log2f(lsum)) * 0.6931471805599453f;
   }
@@ -180,23 +211,30 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 
 // =====================================================================================================
 // Backward.  One CTA per (128-row kv block j, batch, head); two warpgroups own 64 kv rows each and loop over 64-row query
-// blocks i (those that see block j when causal), streamed by a producer warp.  Per warpgroup and block:
+// blocks i (those that see block j when causal), streamed by the producer.  Per warpgroup and block:
 //   S^T = K Q^T, dP^T = V dO^T                      wgmma m64n64k16, both operands K-major in smem
 //   P^T = exp2(S^T c - lse), dS^T = P^T (dP^T - delta)          in registers
-//   dV += P^T dO, dK += dS^T Q                      wgmma with A from registers, B (dO / Q) MN-major in smem
+//   dV += P^T dO, dK += dS^T Q                      wgmma m64nDk16 with A from registers, B (dO / Q) MN-major in smem
 //   dQ  = dS K over this warpgroup's 64 kv rows      dS^T goes through smem (read as an MN-major A operand) ->
-//                                                   fp32 red.add into dq_acc (summed over kv blocks / warpgroups)
+//                                                   fp32 red.add into dq_acc (summed over kv blocks / warpgroups),
+//                                                   one 64-column half of D at a time (keeps D = 128 within 240 registers)
 // =====================================================================================================
 constexpr int BQB = 64;                          // query rows per backward iteration
-constexpr int QB_BYTES = BQB * HD * 2;           // 8 KB
-constexpr int Q_STAGES = 3;
-constexpr int SB_K = 0;
-constexpr int SB_V = SB_K + TILE_BYTES;
-constexpr int SB_DS = SB_V + TILE_BYTES;         // dS^T [128 kv][64 q] bf16, SW128
-constexpr int SB_Q = SB_DS + TILE_BYTES;         // [Q_STAGES]
-constexpr int SB_DO = SB_Q + Q_STAGES * QB_BYTES;
-constexpr int SB_BAR = SB_DO + Q_STAGES * QB_BYTES;
-constexpr int BWD_SMEM = SB_BAR + 256 + 1024;
+
+template <int HD>
+struct BwdSmem {
+  static constexpr int KV_BYTES = 128 * HD * 2;   // K or V: [128 kv x HD]
+  static constexpr int DS_BYTES = 128 * 64 * 2;   // dS^T [128 kv][64 q] bf16, SW128
+  static constexpr int QB_BYTES = BQB * HD * 2;   // Q or dO: [64 q x HD]
+  static constexpr int QB_CHUNK = BQB * 128;      // 8 KB: one [64 x 64] column chunk
+  static constexpr int SB_K = 0;
+  static constexpr int SB_V = SB_K + KV_BYTES;
+  static constexpr int SB_DS = SB_V + KV_BYTES;
+  static constexpr int SB_Q = SB_DS + DS_BYTES;   // [Q_STAGES]
+  static constexpr int SB_DO = SB_Q + AttnCfg<HD>::Q_STAGES * QB_BYTES;
+  static constexpr int SB_BAR = SB_DO + AttnCfg<HD>::Q_STAGES * QB_BYTES;
+  static constexpr int BYTES = SB_BAR + 256 + 1024;
+};
 
 struct AttnBwdParams {
   const float* lse;    // [B,H,S]
@@ -209,13 +247,17 @@ struct AttnBwdParams {
   float scale_log2, scale;
 };
 
-__global__ void __launch_bounds__(THREADS, 1)
+template <int HD>
+__global__ void __launch_bounds__(AttnCfg<HD>::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
                 const AttnBwdParams p) {
+  using L = BwdSmem<HD>;
+  constexpr int Q_STAGES = AttnCfg<HD>::Q_STAGES;
+  constexpr int NC = HD / 64;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SB_BAR);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::SB_BAR);
   uint64_t* kv_full = bars;
   uint64_t* q_full = bars + 1;              // [Q_STAGES]
   uint64_t* q_empty = bars + 1 + Q_STAGES;  // [Q_STAGES]
@@ -243,49 +285,57 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   __syncthreads();
   pdl_wait();
 
-  if (warp == 8) {
-    if (lane == 0) {
-      mbar_expect_tx(kv_full, 2 * TILE_BYTES);
-      tma_load_4d(smem + SB_K, &tmap_k, kv_full, 0, j * BKV, h, b);
-      tma_load_4d(smem + SB_V, &tmap_v, kv_full, 0, j * BKV, h, b);
+  if (HD == 64 ? warp == 8 : warp >= 8) {   // producer: warp 8 (D = 64) / warpgroup 2 (D = 128)
+    if constexpr (HD == 128) setmaxnreg_dec<24>();
+    if (lane == 0 && (HD == 64 || warp == 8)) {
+      mbar_expect_tx(kv_full, 2 * L::KV_BYTES);
+#pragma unroll
+      for (int c = 0; c < NC; ++c) tma_load_4d(smem + L::SB_K + c * CHUNK, &tmap_k, kv_full, c * 64, j * BKV, h, b);
+#pragma unroll
+      for (int c = 0; c < NC; ++c) tma_load_4d(smem + L::SB_V + c * CHUNK, &tmap_v, kv_full, c * 64, j * BKV, h, b);
       for (int i = i0, it = 0; i < nqb; ++i, ++it) {
         const int st = it % Q_STAGES;
         mbar_wait(&q_empty[st], ((it / Q_STAGES) & 1) ^ 1);
-        mbar_expect_tx(&q_full[st], 2 * QB_BYTES);
-        tma_load_4d(smem + SB_Q + st * QB_BYTES, &tmap_q, &q_full[st], 0, i * BQB, h, b);
-        tma_load_4d(smem + SB_DO + st * QB_BYTES, &tmap_do, &q_full[st], 0, i * BQB, h, b);
+        mbar_expect_tx(&q_full[st], 2 * L::QB_BYTES);
+#pragma unroll
+        for (int c = 0; c < NC; ++c)
+          tma_load_4d(smem + L::SB_Q + st * L::QB_BYTES + c * L::QB_CHUNK, &tmap_q, &q_full[st], c * 64, i * BQB, h, b);
+#pragma unroll
+        for (int c = 0; c < NC; ++c)
+          tma_load_4d(smem + L::SB_DO + st * L::QB_BYTES + c * L::QB_CHUNK, &tmap_do, &q_full[st], c * 64, i * BQB, h, b);
       }
     }
     pdl_trigger();
     return;
   }
+  if constexpr (HD == 128) setmaxnreg_inc<240>();
 
   const int wg = warp >> 2;
   const int g = lane >> 2, q = lane & 3;
   const int r0 = (warp & 3) * 16 + g;      // fragment row inside the warpgroup's 64 rows (+8 for e >= 2)
-  const uint32_t sk = smem_u32(smem + SB_K) + wg * 64 * 128, sv = smem_u32(smem + SB_V) + wg * 64 * 128;
-  uint8_t* ds_tile = smem + SB_DS + wg * 64 * 128;   // this warpgroup's 64 kv rows of dS^T
+  const uint32_t sk = smem_u32(smem + L::SB_K) + wg * 64 * 128, sv = smem_u32(smem + L::SB_V) + wg * 64 * 128;
+  uint8_t* ds_tile = smem + L::SB_DS + wg * 64 * 128;   // this warpgroup's 64 kv rows of dS^T
   const uint32_t sds = smem_u32(ds_tile);
   const float* lse_bh = p.lse + ((size_t)b * p.H + h) * p.S;
   const float* delta_bh = p.delta + ((size_t)b * p.H + h) * p.S;
-  float dv[32], dk[32];
+  float dv[HD / 2], dk[HD / 2];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  for (int i = 0; i < HD / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
   mbar_wait(kv_full, 0);
   for (int i = i0, it = 0; i < nqb; ++i, ++it) {
     const int st = it % Q_STAGES;
     mbar_wait(&q_full[st], (it / Q_STAGES) & 1);
-    const uint32_t sq = smem_u32(smem + SB_Q + st * QB_BYTES), sdo = smem_u32(smem + SB_DO + st * QB_BYTES);
+    const uint32_t sq = smem_u32(smem + L::SB_Q + st * L::QB_BYTES), sdo = smem_u32(smem + L::SB_DO + st * L::QB_BYTES);
     float s[32], dp[32];
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
-      wgmma_m64n64k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sk + k * 32, 0, 1024), make_smem_desc_sw128(sq + k * 32, 0, 1024),
-                                    k > 0 ? 1u : 0u);
+    for (int k = 0; k < HD / 16; ++k)
+      wgmma_m64n64k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sk + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024),
+                                    make_smem_desc_sw128(sq + (k / 4) * L::QB_CHUNK + (k % 4) * 32, 0, 1024), k > 0 ? 1u : 0u);
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
-      wgmma_m64n64k16_bf16_ss<0, 0>(dp, make_smem_desc_sw128(sv + k * 32, 0, 1024), make_smem_desc_sw128(sdo + k * 32, 0, 1024),
-                                    k > 0 ? 1u : 0u);
+    for (int k = 0; k < HD / 16; ++k)
+      wgmma_m64n64k16_bf16_ss<0, 0>(dp, make_smem_desc_sw128(sv + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024),
+                                    make_smem_desc_sw128(sdo + (k / 4) * L::QB_CHUNK + (k % 4) * 32, 0, 1024), k > 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(s);
@@ -296,12 +346,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
       for (int e1 = 0; e1 < 2; ++e1) {
         const int qt = 8 * jj + 2 * q + e1;
-        const float L = __ldg(lse_bh + i * BQB + qt) * 1.4426950408889634f;
+        const float L2 = __ldg(lse_bh + i * BQB + qt) * 1.4426950408889634f;
         const float dl = __ldg(delta_bh + i * BQB + qt);
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           const int idx = 4 * jj + 2 * hr + e1;
-          float pv = exp2f(s[idx] * p.scale_log2 - L);
+          float pv = exp2f(s[idx] * p.scale_log2 - L2);
           if (masked && i * BQB + qt < j * BKV + wg * 64 + r0 + 8 * hr) pv = 0.f;
           s[idx] = pv;
           dp[idx] = pv * (dp[idx] - dl);
@@ -321,39 +371,46 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     }
     fence_proxy_async();
     named_bar_sync(1 + wg, 128);
-    float dq[32];
     wgmma_fence();
+    // dO / Q MN-major: LBO = the next 64-column chunk (the field is unused at N = 64)
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
       uint32_t a[4];
       frag_a_from_acc(s, kk, a);
-      wgmma_m64n64k16_bf16_rs<1>(dv, a, make_smem_desc_sw128(sdo + kk * 16 * 128, 8192, 1024), 1u);
+      wgmma_m64nXk16_bf16_rs<1>(dv, a, make_smem_desc_sw128(sdo + kk * 16 * 128, L::QB_CHUNK, 1024), 1u);
     }
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
       uint32_t a[4];
       frag_a_from_acc(dp, kk, a);
-      wgmma_m64n64k16_bf16_rs<1>(dk, a, make_smem_desc_sw128(sq + kk * 16 * 128, 8192, 1024), 1u);
+      wgmma_m64nXk16_bf16_rs<1>(dk, a, make_smem_desc_sw128(sq + kk * 16 * 128, L::QB_CHUNK, 1024), 1u);
     }
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk)
-      wgmma_m64n64k16_bf16_ss<1, 1>(dq, make_smem_desc_sw128(sds + kk * 16 * 128, 8192, 1024),
-                                    make_smem_desc_sw128(sk + kk * 16 * 128, 8192, 1024), kk > 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(dv);
-    fence_regs(dk);
-    fence_regs(dq);
-    if ((threadIdx.x & 127) == 0) mbar_arrive(&q_empty[st]);
+    for (int n = 0; n < NC; ++n) {   // dQ columns [64 n, 64 n + 64); the first half shares the dV / dK commit group
+      float dq[32];
+      if (n > 0) wgmma_fence();
 #pragma unroll
-    for (int hr = 0; hr < 2; ++hr) {
-      const int row = i * BQB + r0 + 8 * hr;
-      float* dqp = p.dq_acc + (((size_t)b * p.S + row) * p.H + h) * HD;
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_m64n64k16_bf16_ss<1, 1>(dq, make_smem_desc_sw128(sds + kk * 16 * 128, 8192, 1024),
+                                      make_smem_desc_sw128(sk + n * CHUNK + kk * 16 * 128, 8192, 1024), kk > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      if (n == 0) {
+        fence_regs(dv);
+        fence_regs(dk);
+      }
+      fence_regs(dq);
+      if (n == 0 && (threadIdx.x & 127) == 0) mbar_arrive(&q_empty[st]);
 #pragma unroll
-      for (int jj = 0; jj < 8; ++jj)
-        asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dqp + 8 * jj + 2 * q), "f"(dq[4 * jj + 2 * hr] * p.scale),
-                     "f"(dq[4 * jj + 2 * hr + 1] * p.scale)
-                     : "memory");
+      for (int hr = 0; hr < 2; ++hr) {
+        const int row = i * BQB + r0 + 8 * hr;
+        float* dqp = p.dq_acc + (((size_t)b * p.S + row) * p.H + h) * HD + n * 64;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dqp + 8 * jj + 2 * q), "f"(dq[4 * jj + 2 * hr] * p.scale),
+                       "f"(dq[4 * jj + 2 * hr + 1] * p.scale)
+                       : "memory");
+      }
     }
   }
   pdl_trigger();
@@ -364,19 +421,22 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     __nv_bfloat16* dkp = reinterpret_cast<__nv_bfloat16*>(p.dk) + off;
     __nv_bfloat16* dvp = reinterpret_cast<__nv_bfloat16*>(p.dv) + off;
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
+    for (int jj = 0; jj < HD / 8; ++jj) {
       *reinterpret_cast<uint32_t*>(dkp + 8 * jj + 2 * q) = pack_bf16x2(dk[4 * jj + 2 * hr] * p.scale, dk[4 * jj + 2 * hr + 1] * p.scale);
       *reinterpret_cast<uint32_t*>(dvp + 8 * jj + 2 * q) = pack_bf16x2(dv[4 * jj + 2 * hr], dv[4 * jj + 2 * hr + 1]);
     }
   }
 }
 
-// delta[b,h,s] = sum_d dO * O ; 8 lanes per (b, s, h) row of 64 elements (one 16-byte load per lane and tensor).
+// delta[b,h,s] = sum_d dO * O ; HD / 8 lanes per (b, s, h) row (one 16-byte load per lane and tensor).
+template <int HD>
 __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ dO, const __nv_bfloat16* __restrict__ O,
                                   float* __restrict__ delta, int B, int S, int H) {
+  constexpr int LANES = HD / 8, LANES_LOG2 = HD == 64 ? 3 : 4;
+  static_assert(LANES == 1 << LANES_LOG2, "HD = 64 or 128");
   const long long gid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  const long long row = gid >> 3;
-  const int sub = (int)(gid & 7);
+  const long long row = gid >> LANES_LOG2;
+  const int sub = (int)(gid & (LANES - 1));
   pdl_wait();
   if (row >= (long long)B * S * H) return;
   const int hh = row % H, s = (row / H) % S, bb = row / ((long long)H * S);
@@ -390,14 +450,14 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ dO, const __
     float2 fa = __bfloat1622float2(ha[i]), fc = __bfloat1622float2(hc[i]);
     v += fa.x * fc.x + fa.y * fc.y;
   }
-  v += __shfl_xor_sync(0xffffffffu, v, 4);
-  v += __shfl_xor_sync(0xffffffffu, v, 2);
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
+#pragma unroll
+  for (int off = LANES / 2; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
   if (sub == 0) delta[((size_t)bb * H + hh) * S + s] = v;
 }
 
 // dq (bf16, strided) = dq_acc (fp32 contiguous [B,S,H,D])
 // (the accumulator is zeroed again on the way out, so the persistent workspace never needs a separate memset)
+template <int HD>
 __global__ void attn_dq_cast_kernel(float* __restrict__ acc, __nv_bfloat16* __restrict__ dq, int B, int S, int H,
                                     long long sb, long long ss, long long sh) {
   const size_t n8 = (size_t)B * S * H * (HD / 8);
@@ -449,47 +509,88 @@ extern "C" int tepd_make_tmap_bshd(CUtensorMap* out, const void* ptr, int B, int
   return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
-// q, k, v: bf16 pointers addressed as [B, S, H, D] with the given element strides (shared by q/k/v).
-extern "C" int tepd_attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, int B, int H, int S, int D,
-                             float scale, int causal, long long stride_b, long long stride_s, long long stride_h,
-                             void* stream) {
-  if (D != HD || S % 128 != 0) return -2;
+namespace {
+
+template <int HD>
+int attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, int B, int H, int S, float scale, int causal,
+             long long stride_b, long long stride_s, long long stride_h, cudaStream_t stream) {
   CUtensorMap tq, tk, tv;
-  int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, D, stride_b, stride_s, stride_h, BQ);
+  int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, HD, stride_b, stride_s, stride_h, BQ);
   if (rc) return 100 + rc;
-  rc = tepd_make_tmap_bshd(&tk, k, B, S, H, D, stride_b, stride_s, stride_h, BKV);
+  rc = tepd_make_tmap_bshd(&tk, k, B, S, H, HD, stride_b, stride_s, stride_h, BKV);
   if (rc) return 200 + rc;
-  rc = tepd_make_tmap_bshd(&tv, v, B, S, H, D, stride_b, stride_s, stride_h, BKV);
+  rc = tepd_make_tmap_bshd(&tv, v, B, S, H, HD, stride_b, stride_s, stride_h, BKV);
   if (rc) return 300 + rc;
   static bool cfg = false;
   if (!cfg) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FWD_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem<HD>::BYTES);
     if (e != cudaSuccess) return (int)e;
     cfg = true;
   }
   AttnFwdParams p;
   p.O = o; p.lse = (float*)lse; p.B = B; p.H = H; p.S = S; p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
-  return (int)tepd::launch(attn_fwd_kernel, dim3((S / BQ) * B * H), dim3(THREADS), FWD_SMEM, reinterpret_cast<cudaStream_t>(stream),
+  return (int)tepd::launch(attn_fwd_kernel<HD>, dim3((S / BQ) * B * H), dim3(AttnCfg<HD>::THREADS), FwdSmem<HD>::BYTES, stream,
                            tq, tk, tv, p);
 }
 
-// do, o: contiguous [B,S,H,D]; q/k/v strided views; dq/dk/dv strided views (shared strides).
+template <int HD>
+int attn_bwd(const void* dO, const void* q, const void* k, const void* v, const void* o, const void* lse, float* delta,
+             float* dq_acc, void* dq, void* dk, void* dv, int B, int H, int S, float scale, int causal, long long stride_b,
+             long long stride_s, long long stride_h, long long dstride_b, long long dstride_s, long long dstride_h,
+             cudaStream_t st) {
+  CUtensorMap tq, tk, tv, tdo;
+  int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, HD, stride_b, stride_s, stride_h, BQB);
+  if (rc) return 100 + rc;
+  rc = tepd_make_tmap_bshd(&tk, k, B, S, H, HD, stride_b, stride_s, stride_h, BKV);
+  if (rc) return 200 + rc;
+  rc = tepd_make_tmap_bshd(&tv, v, B, S, H, HD, stride_b, stride_s, stride_h, BKV);
+  if (rc) return 300 + rc;
+  rc = tepd_make_tmap_bshd(&tdo, dO, B, S, H, HD, (long long)S * H * HD, (long long)H * HD, HD, BQB);
+  if (rc) return 400 + rc;
+  {
+    const long long rows = (long long)B * S * H;
+    cudaError_t le = tepd::launch(attn_delta_kernel<HD>, dim3((unsigned)((rows * (HD / 8) + 255) / 256)), dim3(256), 0, st,
+                                  (const __nv_bfloat16*)dO, (const __nv_bfloat16*)o, delta, B, S, H);
+    if (le != cudaSuccess) return (int)le;
+  }
+  static bool cfg = false;
+  if (!cfg) {
+    cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem<HD>::BYTES);
+    if (e != cudaSuccess) return (int)e;
+    cfg = true;
+  }
+  AttnBwdParams p;
+  p.lse = (const float*)lse; p.delta = delta; p.dq_acc = dq_acc; p.dk = dk; p.dv = dv;
+  p.dstride_b = dstride_b; p.dstride_s = dstride_s; p.dstride_h = dstride_h;
+  p.B = B; p.H = H; p.S = S; p.causal = causal; p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
+  cudaError_t le = tepd::launch(attn_bwd_kernel<HD>, dim3((S / BKV) * B * H), dim3(AttnCfg<HD>::THREADS), BwdSmem<HD>::BYTES, st,
+                                tq, tk, tv, tdo, p);
+  if (le != cudaSuccess) return (int)le;
+  return (int)tepd::launch(attn_dq_cast_kernel<HD>, dim3(tepd::num_sms() * 4), dim3(256), 0, st, dq_acc, (__nv_bfloat16*)dq, B, S,
+                           H, dstride_b, dstride_s, dstride_h);
+}
+
+}  // namespace
+
+// q, k, v: bf16 pointers addressed as [B, S, H, D] with the given element strides (shared by q/k/v).  D = 64 or 128.
+extern "C" int tepd_attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, int B, int H, int S, int D,
+                             float scale, int causal, long long stride_b, long long stride_s, long long stride_h,
+                             void* stream) {
+  if (S % 128 != 0) return -2;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (D == 64) return attn_fwd<64>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, st);
+  if (D == 128) return attn_fwd<128>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, st);
+  return -2;
+}
+
+// do, o: contiguous [B,S,H,D]; q/k/v strided views; dq/dk/dv strided views (shared strides).  D = 64 or 128.
 extern "C" int tepd_attn_bwd(const void* dO, const void* q, const void* k, const void* v, const void* o, const void* lse,
                              void* dq_acc, void* dq, void* dk, void* dv, int B, int H, int S, int D, float scale,
                              int causal, long long stride_b, long long stride_s, long long stride_h, long long dstride_b,
                              long long dstride_s, long long dstride_h, void* stream) {
-  if (D != HD || S % 128 != 0) return -2;
+  if ((D != 64 && D != 128) || S % 128 != 0) return -2;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CUtensorMap tq, tk, tv, tdo;
-  int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, D, stride_b, stride_s, stride_h, BQB);
-  if (rc) return 100 + rc;
-  rc = tepd_make_tmap_bshd(&tk, k, B, S, H, D, stride_b, stride_s, stride_h, BKV);
-  if (rc) return 200 + rc;
-  rc = tepd_make_tmap_bshd(&tv, v, B, S, H, D, stride_b, stride_s, stride_h, BKV);
-  if (rc) return 300 + rc;
-  rc = tepd_make_tmap_bshd(&tdo, dO, B, S, H, D, (long long)S * H * D, (long long)H * D, D, BQB);
-  if (rc) return 400 + rc;
   static float* delta_buf = nullptr;
   static size_t delta_cap = 0;
   const size_t need = (size_t)B * H * S;
@@ -498,17 +599,11 @@ extern "C" int tepd_attn_bwd(const void* dO, const void* q, const void* k, const
     if (cudaMalloc(&delta_buf, need * sizeof(float)) != cudaSuccess) return -5;
     delta_cap = need;
   }
-  {
-    const long long rows = (long long)B * S * H;
-    cudaError_t le = tepd::launch(attn_delta_kernel, dim3((unsigned)((rows * 8 + 255) / 256)), dim3(256), 0, st,
-                                  (const __nv_bfloat16*)dO, (const __nv_bfloat16*)o, delta_buf, B, S, H);
-    if (le != cudaSuccess) return (int)le;
-  }
   // persistent, self-clearing fp32 dQ accumulator (used when the caller passes no buffer)
   static float* dq_ws = nullptr;
   static size_t dq_cap = 0;
   if (dq_acc == nullptr) {
-    const size_t needq = (size_t)B * S * H * HD;
+    const size_t needq = (size_t)B * S * H * D;
     if (needq > dq_cap) {
       if (dq_ws) cudaFree(dq_ws);
       if (cudaMalloc(&dq_ws, needq * sizeof(float)) != cudaSuccess) return -6;
@@ -517,18 +612,9 @@ extern "C" int tepd_attn_bwd(const void* dO, const void* q, const void* k, const
     }
     dq_acc = dq_ws;
   }
-  static bool cfg = false;
-  if (!cfg) {
-    cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
-    if (e != cudaSuccess) return (int)e;
-    cfg = true;
-  }
-  AttnBwdParams p;
-  p.lse = (const float*)lse; p.delta = delta_buf; p.dq_acc = (float*)dq_acc; p.dk = dk; p.dv = dv;
-  p.dstride_b = dstride_b; p.dstride_s = dstride_s; p.dstride_h = dstride_h;
-  p.B = B; p.H = H; p.S = S; p.causal = causal; p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
-  cudaError_t le = tepd::launch(attn_bwd_kernel, dim3((S / BKV) * B * H), dim3(THREADS), BWD_SMEM, st, tq, tk, tv, tdo, p);
-  if (le != cudaSuccess) return (int)le;
-  return (int)tepd::launch(attn_dq_cast_kernel, dim3(tepd::num_sms() * 4), dim3(256), 0, st, (float*)dq_acc, (__nv_bfloat16*)dq, B, S, H,
-                           dstride_b, dstride_s, dstride_h);
+  if (D == 64)
+    return attn_bwd<64>(dO, q, k, v, o, lse, delta_buf, (float*)dq_acc, dq, dk, dv, B, H, S, scale, causal, stride_b, stride_s,
+                        stride_h, dstride_b, dstride_s, dstride_h, st);
+  return attn_bwd<128>(dO, q, k, v, o, lse, delta_buf, (float*)dq_acc, dq, dk, dv, B, H, S, scale, causal, stride_b, stride_s,
+                       stride_h, dstride_b, dstride_s, dstride_h, st);
 }
