@@ -92,39 +92,6 @@ __device__ __forceinline__ void next_work(const GemmParams& p, int& cursor, int 
   }
 }
 
-// Peer-memory fusion (tensor parallel):
-//   mode 1  GEMM -> reduce-scatter : output rows [r*rows_per_owner, (r+1)*rows_per_owner) are reduced into rank r's fp32
-//           buffer with red.add over NVLink straight from the epilogue (no separate collective, overlaps tile by tile)
-//   mode 2  all-gather -> GEMM     : A rows are fetched by TMA directly from the rank that owns them (peer-mapped shards)
-//   mode 3  GEMM -> reduce-scatter : partial rows are written as bf16 with plain 16-byte stores into slot [src rank] of the
-//           owner's staging buffer (no atomics on the wire); slot_reduce (comm_sm90.cu) sums the n slots on the owner
-//   mode 4  all-gather -> GEMM     : a concurrent copy kernel (p2p_gather_chunks) pulls the peers' shards into a local
-//           staging buffer chunk by chunk and publishes a flag per chunk; the TMA producer starts on the local shard and
-//           waits on a chunk's flag just before its first tile of that chunk, so the NVLink transfer hides under the MMAs
-// Peer tiles are walked chunk-major (own rows first, then rank+1's, ...), so at any moment the n ranks talk to n
-// different peers and mode 4 meets its chunks in the order the copy kernel delivers them.
-constexpr int MAX_PEERS = 8;
-struct PeerArgs {
-  int mode, n, rank, rows_per_owner;
-  void* out[MAX_PEERS];
-  const uint32_t* flags;  // mode 4: flags[owner] == *epoch once owner's rows are staged locally
-  const uint32_t* epoch;
-};
-
-__device__ __forceinline__ void peer_tile(const PeerArgs* pa, int m_blocks, int n_blocks, int tile, int& m_blk, int& n_blk) {
-  const int mpc = m_blocks / pa->n;  // m-blocks per owner chunk
-  const int per_chunk = mpc * n_blocks;
-  const int chunk = tile / per_chunk;
-  const int rem = tile - chunk * per_chunk;
-  n_blk = rem / mpc;
-  int owner = pa->rank + chunk;
-  if (owner >= pa->n) owner -= pa->n;
-  m_blk = owner * mpc + (rem - n_blk * mpc);
-}
-struct TmapArray {
-  CUtensorMap m[MAX_PEERS];
-};
-
 __device__ __forceinline__ float gelu_tanh_grad(float x) {
   const float k0 = 0.7978845608028654f, k1 = 0.044715f;
   float t;
@@ -155,9 +122,8 @@ __device__ __forceinline__ float2 ld_bf16x2(const void* p) {
 
 // Epilogue math + store for two adjacent columns (col, col + 1) of one output row.  v0 / v1 already hold the scaled
 // accumulator.  N % 8 == 0 and col is even, so col < N covers both columns.
-template <bool PEER>
-__device__ __forceinline__ void epilogue_pair(float v0, float v1, const GemmParams& p, const PeerArgs* pa, int row, int col, int b,
-                                              bool add_bias, bool add_res) {
+__device__ __forceinline__ void epilogue_pair(float v0, float v1, const GemmParams& p, int row, int col, int b, bool add_bias,
+                                              bool add_res) {
   if (add_bias) {
     if (p.bias_bf16) {
       const float2 f = ld_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.bias) + (long long)b * p.bias_stride + col);
@@ -182,24 +148,11 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, const GemmPara
   }
   if (!p.out_fp32) {
     __nv_bfloat16* dp = reinterpret_cast<__nv_bfloat16*>(p.D2 != nullptr && p.act == 1 ? p.D2 : p.D) + off;
-    if constexpr (PEER) {
-      if (pa->mode == 3) {  // partial rows -> slot [my rank] of the owner's staging buffer (plain stores over NVLink)
-        const int owner = row / pa->rows_per_owner;
-        dp = reinterpret_cast<__nv_bfloat16*>(pa->out[owner]) +
-             ((long long)pa->rank * pa->rows_per_owner + (row - owner * pa->rows_per_owner)) * p.ldd + col;
-      }
-    }
     st_bf16x2(dp, v0, v1);
   } else if (!p.accumulate) {
     *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.D) + off) = make_float2(v0, v1);
   } else {
     float* dp = reinterpret_cast<float*>(p.D) + off;
-    if constexpr (PEER) {
-      if (pa->mode == 1) {  // reduce-scatter: this row belongs to rank `owner`; add into ITS buffer over NVLink
-        const int owner = row / pa->rows_per_owner;
-        dp = reinterpret_cast<float*>(pa->out[owner]) + (long long)(row - owner * pa->rows_per_owner) * p.ldd + col;
-      }
-    }
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dp), "f"(v0), "f"(v1) : "memory");
   }
 }
@@ -227,9 +180,8 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 128][64], uint
 
 // Warp roles: warps 0-7 = two consumer warpgroups (wgmma into registers, rows [64 wg, +64) of the 128-row tile, then the
 // epilogue straight from the accumulator fragments); warp 8 = TMA producer.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool PEER, bool FP8>
-__device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmParams& p,
-                                          const PeerArgs* pa, const TmapArray* tmaps_a) {
+template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmParams& p) {
   using C = Cfg<BLOCK_N>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -257,52 +209,21 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
     if (elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      int peer_ready = -1;
-      (void)peer_ready;
       int cursor, cend;
       work_range(p, cursor, cend);
       while (cursor < cend) {
-        const int tile = cursor;
         Work w;
         next_work(p, cursor, cend, w);
-        int m_blk = w.m_blk, n_blk = w.n_blk;
+        const int m_blk = w.m_blk, n_blk = w.n_blk;
         const int b = w.b, kb0 = w.kb0, kb1 = w.kb1;
-        const CUtensorMap* ta = &tmap_a;
-        int a_row = m_blk * BLOCK_M;
-        if constexpr (PEER) {
-          peer_tile(pa, p.m_blocks, p.n_blocks, tile, m_blk, n_blk);
-          a_row = m_blk * BLOCK_M;
-          if (pa->mode == 2) {
-            const int owner = a_row / pa->rows_per_owner;
-            ta = &tmaps_a->m[owner];
-            a_row -= owner * pa->rows_per_owner;
-          } else if (pa->mode == 4) {
-            const int owner = a_row / pa->rows_per_owner;
-            if (owner == pa->rank) {  // own shard: read it where it lives
-              a_row -= owner * pa->rows_per_owner;
-            } else {                  // staged copy of a peer's shard: wait until the copy kernel published it
-              ta = &tmaps_a->m[(pa->rank + 1) % pa->n];
-              if (owner != peer_ready) {
-                const uint32_t want = *reinterpret_cast<const volatile uint32_t*>(pa->epoch);
-                uint32_t got;
-                const long long t0 = clock64();
-                do {
-                  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(got) : "l"(pa->flags + owner) : "memory");
-                  if (got != want && clock64() - t0 > 4000000000LL) __trap();  // copy kernel never ran: fail loudly, don't hang
-                } while (got != want);
-                asm volatile("fence.proxy.async;" ::: "memory");
-                peer_ready = owner;
-              }
-            }
-          }
-        }
+        const int a_row = m_blk * BLOCK_M;
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * C::STAGE_BYTES;
           uint8_t* sb = sa + C::A_BYTES;
           mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
           if constexpr (!A_MN) {
-            tma_load_3d(sa, ta, &full_bar[stage], kb * BLOCK_K * (FP8 ? 2 : 1), a_row, b);
+            tma_load_3d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K * (FP8 ? 2 : 1), a_row, b);
           } else {
 #pragma unroll
             for (int j = 0; j < BLOCK_M / 64; ++j)
@@ -335,10 +256,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
       const int tile = cursor;
       Work w;
       next_work(p, cursor, cend, w);
-      int m_blk = w.m_blk, n_blk = w.n_blk;
+      const int m_blk = w.m_blk, n_blk = w.n_blk;
       const int b = w.b;
       const bool has_k = w.kb0 < w.kb1;
-      if constexpr (PEER) peer_tile(pa, p.m_blocks, p.n_blocks, tile, m_blk, n_blk);
       float acc[BLOCK_N / 128][64];
       int prev = -1;
       for (int kb = w.kb0; kb < w.kb1; ++kb) {
@@ -414,7 +334,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
                   v0 += t.x; v1 += t.y;
                 }
               }
-              epilogue_pair<PEER>(v0, v1, p, pa, row, col, b, add_bias, add_res);
+              epilogue_pair(v0, v1, p, row, col, b, add_bias, add_res);
             }
           }
         }
@@ -438,14 +358,7 @@ template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const GemmParams p) {
-  gemm_body<BLOCK_N, A_MN, B_MN, false, FP8>(tmap_a, tmap_b, p, nullptr, nullptr);
-}
-
-template <int BLOCK_N, bool B_MN>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_bf16_peer_kernel(const __grid_constant__ TmapArray tmaps_a, const __grid_constant__ CUtensorMap tmap_b,
-                      const GemmParams p, const __grid_constant__ PeerArgs pa) {
-  gemm_body<BLOCK_N, false, B_MN, true, false>(tmaps_a.m[pa.rank], tmap_b, p, &pa, &tmaps_a);
+  gemm_body<BLOCK_N, A_MN, B_MN, FP8>(tmap_a, tmap_b, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -600,74 +513,6 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
   return launch_gemm<BN, true, true>(ta, tb, p, num_sms, s);
   if (block_n == 256) { DISPATCH(256) } else { DISPATCH(128) }
 #undef DISPATCH
-}
-
-
-template <int BLOCK_N, bool B_MN>
-static int launch_gemm_peer(const TmapArray& ta, const CUtensorMap& tb, const GemmParams& p, const PeerArgs& pa, int num_sms,
-                            cudaStream_t stream) {
-  using C = Cfg<BLOCK_N>;
-  auto kern = gemm_bf16_peer_kernel<BLOCK_N, B_MN>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
-  int total = p.m_blocks * p.n_blocks * p.batch * p.split_k;
-  int grid = total < num_sms ? total : num_sms;
-  return (int)tepd::launch(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, ta, tb, p, pa);
-}
-
-// Tensor-parallel fused GEMMs over peer memory.
-//   mode 1 (GEMM -> reduce-scatter): A [M, K_local] local, B local; out_ptrs[r] = rank r's fp32 [M/n, N] buffer (pre-zeroed).
-//   mode 2 (all-gather -> GEMM)    : a_ptrs[r] = rank r's bf16 shard [M/n, K]; D local [M, N] (bf16 or fp32).
-//   mode 3 (GEMM -> reduce-scatter): as mode 1 but out_ptrs[r] = rank r's bf16 slot buffer [n, M/n, N]; follow with slot_reduce.
-//   mode 4 (all-gather -> GEMM)    : a_ptrs[rank] = own shard [M/n, K]; a_ptrs[(rank+1)%n] = local staging buffer [M, K] that
-//                                    p2p_gather_chunks fills; flags / epoch as published by that kernel.
-extern "C" int tepd_gemm_bf16_peer(int mode, void* const* a_ptrs, const void* B, void* D, void* const* out_ptrs, const void* bias,
-                                   int M, int N, int K, long long lda, long long ldb, long long ldd, int b_mn, int out_fp32,
-                                   int n_peers, int rank, int block_n, int num_sms, void* stream, const void* flags,
-                                   const void* epoch) {
-  if (N % 8 != 0 || K % 8 != 0 || n_peers < 1 || n_peers > MAX_PEERS || M % n_peers) return -2;
-  const int rows_per_owner = M / n_peers;
-  if (rows_per_owner % BLOCK_M) return -3;
-  GemmParams p;
-  p.M = M; p.N = N; p.K = K; p.batch = 1;
-  if (block_n != 128 && block_n != 256) block_n = (N % 256 == 0 || N > 1024) ? 256 : 128;
-  p.m_blocks = M / BLOCK_M;
-  p.n_blocks = (N + block_n - 1) / block_n;
-  p.k_blocks = (K + BLOCK_K - 1) / BLOCK_K;
-  p.split_k = 1; p.stream_k = 0; p.sk_ws = nullptr; p.sk_cnt = nullptr;
-  p.ldd = ldd; p.stride_d = 0; p.ld_res = 0; p.stride_res = 0;
-  const bool gather = mode == 2 || mode == 4;
-  p.D = D; p.bias = gather ? bias : nullptr; p.residual = nullptr; p.alpha = 1.0f;
-  p.out_fp32 = mode == 1 ? 1 : (mode == 3 ? 0 : out_fp32); p.accumulate = mode == 1 ? 1 : 0; p.act = 0; p.bias_bf16 = 0;
-  p.D2 = nullptr; p.aux = nullptr;
-  p.row_scale = nullptr; p.w_scale = nullptr; p.bias_stride = 0;
-  PeerArgs pa;
-  pa.mode = mode; pa.n = n_peers; pa.rank = rank; pa.rows_per_owner = rows_per_owner;
-  pa.flags = reinterpret_cast<const uint32_t*>(flags); pa.epoch = reinterpret_cast<const uint32_t*>(epoch);
-  if (mode == 4 && n_peers > 1 && (!flags || !epoch)) return -4;
-  for (int i = 0; i < MAX_PEERS; ++i) pa.out[i] = ((mode == 1 || mode == 3) && i < n_peers) ? out_ptrs[i] : nullptr;
-  TmapArray ta;
-  int rc;
-  for (int r = 0; r < n_peers; ++r) {
-    if (mode == 2)      rc = tepd_make_tmap_bf16_3d(&ta.m[r], a_ptrs[r], K, rows_per_owner, 1, lda, 0, BLOCK_K, BLOCK_M);
-    else if (mode == 4) rc = r == rank ? tepd_make_tmap_bf16_3d(&ta.m[r], a_ptrs[r], K, rows_per_owner, 1, lda, 0, BLOCK_K, BLOCK_M)
-                                       : tepd_make_tmap_bf16_3d(&ta.m[r], a_ptrs[(rank + 1) % n_peers], K, M, 1, lda, 0, BLOCK_K, BLOCK_M);
-    else                rc = tepd_make_tmap_bf16_3d(&ta.m[r], a_ptrs[0], K, M, 1, lda, 0, BLOCK_K, BLOCK_M);
-    if (rc) return 100 + rc;
-  }
-  for (int r = n_peers; r < MAX_PEERS; ++r) ta.m[r] = ta.m[0];
-  CUtensorMap tb;
-  if (!b_mn) rc = tepd_make_tmap_bf16_3d(&tb, B, K, N, 1, ldb, 0, BLOCK_K, block_n);
-  else       rc = tepd_make_tmap_bf16_3d(&tb, B, N, K, 1, ldb, 0, 64, BLOCK_K);
-  if (rc) return 200 + rc;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (num_sms <= 0) num_sms = tepd::num_sms();
-  if (block_n == 256) return b_mn ? launch_gemm_peer<256, true>(ta, tb, p, pa, num_sms, s) : launch_gemm_peer<256, false>(ta, tb, p, pa, num_sms, s);
-  return b_mn ? launch_gemm_peer<128, true>(ta, tb, p, pa, num_sms, s) : launch_gemm_peer<128, false>(ta, tb, p, pa, num_sms, s);
 }
 
 // ------------------------------------------------------------------ fp8 (e4m3) grouped GEMM for the MoE experts

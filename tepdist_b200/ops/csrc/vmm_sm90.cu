@@ -11,7 +11,6 @@
 //                           each rank pulls its 1/n slice already reduced by the switch and broadcasts the result
 //     mc_rs_adamw_ag        data-parallel optimizer step over NVLS: gradient reduce-scatter = multimem.ld_reduce (fp32 or
 //                           bf16 wire), AdamW on the owned shard, bf16 parameter all-gather = multimem.st
-//     mc_all_gather         broadcast the owned slice of a symmetric buffer to every rank
 //
 // The reference reaches the same hardware only through NCCL (SURVEY 2.H K1-K3; dapple_all_reduce_thunk.cc:136-159); it has
 // no reduce-scatter and never fuses a collective with the math around it.
@@ -429,21 +428,6 @@ __global__ void __launch_bounds__(256, 2) mc_rs_adamw_ag_kernel(const void* __re
   }
 }
 
-// every rank's buf[begin16:end16) (16-byte units) = this rank's local values
-__global__ void __launch_bounds__(256) mc_all_gather_kernel(const uint4* __restrict__ local, uint4* __restrict__ buf_mc,
-                                                            long long begin16, long long end16) {
-  for (long long i = begin16 + blockIdx.x * (long long)blockDim.x + threadIdx.x; i < end16; i += (long long)gridDim.x * blockDim.x)
-    mm_st_b128(buf_mc + i, local[i]);
-}
-
-// out[begin:end) (local fp32) = sum over ranks of in[begin:end) (fp32 symmetric buffer, multicast view)
-__global__ void __launch_bounds__(256) mc_reduce_scatter_f32_kernel(const float* __restrict__ in_mc, float* __restrict__ out,
-                                                                    long long begin, long long end) {
-  const long long nvec = (end - begin) >> 2;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x)
-    *reinterpret_cast<float4*>(out + begin + (i << 2)) = mm_ld_reduce_f32x4(in_mc + begin + (i << 2));
-}
-
 }  // namespace
 
 #define CS(s) reinterpret_cast<cudaStream_t>(s)
@@ -479,20 +463,5 @@ extern "C" int tepd_mc_rs_adamw_ag(const void* grad_mc, void* param_mc, void* ma
   else
     mc_rs_adamw_ag_kernel<false><<<ctas, 256, 0, CS(stream)>>>(grad_mc, (bf16*)param_mc, (float*)master, (float*)m, (float*)v, begin,
                                                                end, n_decay, b1, b2, eps, wd, (const float*)hyper);
-  return (int)cudaGetLastError();
-}
-
-extern "C" int tepd_mc_all_gather(const void* local, void* buf_mc, long long begin_bytes, long long end_bytes, int ctas,
-                                  void* stream) {
-  if ((begin_bytes & 15) || (end_bytes & 15)) return -2;
-  if (ctas <= 0) ctas = 64;
-  mc_all_gather_kernel<<<ctas, 256, 0, CS(stream)>>>((const uint4*)local, (uint4*)buf_mc, begin_bytes >> 4, end_bytes >> 4);
-  return (int)cudaGetLastError();
-}
-
-extern "C" int tepd_mc_reduce_scatter_f32(const void* in_mc, void* out, long long begin, long long end, int ctas, void* stream) {
-  if ((begin & 3) || (end & 3)) return -2;
-  if (ctas <= 0) ctas = 64;
-  mc_reduce_scatter_f32_kernel<<<ctas, 256, 0, CS(stream)>>>((const float*)in_mc, (float*)out, begin, end);
   return (int)cudaGetLastError();
 }

@@ -27,11 +27,6 @@ def _sigs(lib):
         "tepd_ipc_close": [vp], "tepd_ipc_handle_size": [],
         "tepd_symm_barrier": [pp, i, i, vp, vp],
         "tepd_fused_rs_adamw_ag": [pp, pp, vp, vp, vp, i, ll, ll, ll, f, f, f, f, vp, i, vp, i],
-        "tepd_p2p_reduce_scatter": [pp, vp, i, ll, ll, i, vp],
-        "tepd_p2p_all_gather": [pp, i, i, ll, ll, i, vp],
-        "tepd_slot_reduce": [vp, i, ll, i, vp, vp, vp, vp, i, vp],
-        "tepd_p2p_gather_chunks": [pp, vp, i, i, ll, vp, vp, vp, i, vp],
-        "tepd_slot_reduce_bcast": [vp, i, ll, i, vp, vp, pp, i, i, vp],
     }
     for k, a in table.items():
         fn = getattr(lib, k)
@@ -53,8 +48,6 @@ def _vmm_sigs(lib):
         "tepd_mc_barrier": [vp, vp, vp, i, vp, vp],
         "tepd_mc_all_reduce_bf16": [vp, vp, vp, vp, i, i, ll, i, vp, vp, vp, i, vp],
         "tepd_mc_rs_adamw_ag": [vp, vp, vp, vp, vp, ll, ll, ll, f, f, f, f, vp, i, i, vp],
-        "tepd_mc_all_gather": [vp, vp, ll, ll, i, vp],
-        "tepd_mc_reduce_scatter_f32": [vp, vp, ll, ll, i, vp],
     }
     for k, a in table.items():
         fn = getattr(lib, k)
@@ -373,156 +366,15 @@ class FusedShardedOptimizer:
         ops._count()
 
 
-# ------------------------------------------------------------------------------------------------ tensor-parallel fused GEMMs
-def _peer_sig(lib):
-    vp, i, ll = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong
-    pp = ctypes.POINTER(ctypes.c_void_p)
-    fn = lib.tepd_gemm_bf16_peer
-    fn.restype = ctypes.c_int
-    fn.argtypes = [i, pp, vp, vp, pp, vp, i, i, i, ll, ll, ll, i, i, i, i, i, i, vp, vp, vp]
-
-
-def gemm_reduce_scatter(x: torch.Tensor, w: torch.Tensor, out: SymmetricBuffer, N: int, b_mn: bool = False,
-                        block_n: int = 0) -> torch.Tensor:
-    """Row-parallel linear fused with its reduce-scatter: every rank multiplies its K-shard (x [M, K/n], w [N, K/n]) and
-    the epilogue adds each output row block straight into the OWNER rank's fp32 buffer over NVLink.  `out` is a
-    zero-initialised symmetric fp32 buffer of [M/n, N] per rank; after a barrier the owner holds sum_r x_r w_r^T."""
-    lib = out.lib
-    _peer_sig(lib)
-    M, K = x.shape
-    rc = lib.tepd_gemm_bf16_peer(1, (ctypes.c_void_p * out.world)(*([x.data_ptr()] * out.world)), w.data_ptr(), None, out.ptr_array,
-                                 None, M, N, K, x.stride(0), w.stride(0), N, int(b_mn), 1, out.world, out.rank, block_n,
-                                 ops._sms(), torch.cuda.current_stream().cuda_stream, None, None)
-    if rc:
-        raise RuntimeError(f"gemm_reduce_scatter failed ({rc})")
-    ops._count()
-    return out.tensor(torch.float32, (M // out.world) * N).view(M // out.world, N)
-
-
-def all_gather_gemm(x_shard: SymmetricBuffer, rows_per_rank: int, K: int, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
-                    out_dtype: torch.dtype = torch.bfloat16, b_mn: bool = False, block_n: int = 0) -> torch.Tensor:
-    """Column-parallel linear fused with the all-gather of its input: the activation is row-sharded across ranks
-    (x_shard holds [rows_per_rank, K] bf16 on every rank); TMA loads fetch each A tile from the rank that owns it."""
-    lib = x_shard.lib
-    _peer_sig(lib)
-    n = x_shard.world
-    M = rows_per_rank * n
-    N = w.shape[1] if b_mn else w.shape[0]
-    d = torch.empty(M, N, dtype=out_dtype, device=w.device)
-    rc = lib.tepd_gemm_bf16_peer(2, x_shard.ptr_array, w.data_ptr(), d.data_ptr(), (ctypes.c_void_p * n)(*([None] * n)),
-                                 None if bias is None else bias.data_ptr(), M, N, K, K, w.stride(0), N, int(b_mn),
-                                 int(out_dtype == torch.float32), n, x_shard.rank, block_n, ops._sms(),
-                                 torch.cuda.current_stream().cuda_stream, None, None)
-    if rc:
-        raise RuntimeError(f"all_gather_gemm failed ({rc})")
-    ops._count()
-    return d
-
-
-class GemmReduceScatter:
-    """Row-parallel linear + reduce-scatter without atomics on the wire: the GEMM epilogue writes each bf16 partial row
-    block into slot [my rank] of the OWNER's staging buffer with plain 16-byte NVLink stores (gemm_sm90.cu peer mode 3),
-    one flag barrier later the owner sums its n slots (+ bias + residual) in a single pass (slot_reduce).  Two staging
-    buffers alternate so the barrier that publishes round i also protects the slots of round i-1 from being overwritten
-    early.  Replaces the reference's dot -> in-stream NCCL all-reduce pair (SURVEY 2.H K1; service/gpu/
-    dapple_all_reduce_thunk.cc:60-120)."""
-
-    def __init__(self, M: int, N: int, group=None, barrier: Optional[SymmBarrier] = None):
-        self.M, self.N = M, N
-        self.world = dist.get_world_size(group)
-        self.rank = dist.get_rank(group)
-        self.rows = M // self.world
-        self.slots = [SymmetricBuffer(self.world * self.rows * N * 2, group) for _ in range(2)]
-        self.barrier = barrier or SymmBarrier(group)
-        self.turn = 0
-
-    def __call__(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
-                 residual: Optional[torch.Tensor] = None, out_dtype: torch.dtype = torch.bfloat16, b_mn: bool = False,
-                 block_n: int = 0) -> torch.Tensor:
-        buf = self.slots[self.turn]
-        self.turn ^= 1
-        lib = buf.lib
-        _peer_sig(lib)
-        M, K = x.shape
-        s = torch.cuda.current_stream().cuda_stream
-        rc = lib.tepd_gemm_bf16_peer(3, (ctypes.c_void_p * self.world)(*([x.data_ptr()] * self.world)), w.data_ptr(), None,
-                                     buf.ptr_array, None, M, self.N, K, x.stride(0), w.stride(0), self.N, int(b_mn), 0,
-                                     self.world, self.rank, block_n, ops._sms(), s, None, None)
-        if rc:
-            raise RuntimeError(f"gemm_reduce_scatter(slots) failed ({rc})")
-        ops._count()
-        self.barrier()
-        out = torch.empty(self.rows, self.N, dtype=out_dtype, device=x.device)
-        bf = out_dtype == torch.bfloat16
-        rc = lib.tepd_slot_reduce(buf.local_ptr, self.world, self.rows, self.N, None if bias is None else bias.data_ptr(),
-                                  None if residual is None else residual.data_ptr(), out.data_ptr() if bf else None,
-                                  None if bf else out.data_ptr(), 0, s)
-        if rc:
-            raise RuntimeError(f"slot_reduce failed ({rc})")
-        ops._count()
-        return out
-
-
-class GemmAllReduce:
-    """Row-parallel linear + ALL-reduce in two kernels and two flag barriers, no NCCL: the GEMM epilogue pushes every bf16
-    partial row block into the owner's slot (peer mode 3), the owner sums its slots together with bias + residual and
-    stores the finished rows into EVERY rank's output buffer (slot_reduce with broadcast).  The transfer of partials
-    overlaps the GEMM tile by tile; what is left after the GEMM is one pass over M/n rows.  Replaces the reference's
-    dot -> in-stream ncclAllReduce pair of tensor-parallel plans (dapple_all_reduce_thunk.cc:136-159).
-    One instance serves every call site of a given [M, N] (slot buffers alternate; each call site owns its symmetric
-    output buffer, allocate with `new_output()`)."""
-
-    def __init__(self, M: int, N: int, group=None, barrier: Optional[SymmBarrier] = None):
-        self.M, self.N, self.group = M, N, group
-        self.world = dist.get_world_size(group)
-        self.rank = dist.get_rank(group)
-        assert M % self.world == 0
-        self.rows = M // self.world
-        self.slots = [SymmetricBuffer(self.world * self.rows * N * 2, group) for _ in range(2)]
-        self.barrier = barrier or SymmBarrier(group)
-        self.turn = 0
-
-    def new_output(self) -> SymmetricBuffer:
-        return SymmetricBuffer(self.M * self.N * 2, self.group)
-
-    def __call__(self, x: torch.Tensor, w: torch.Tensor, out: SymmetricBuffer, bias: Optional[torch.Tensor] = None,
-                 residual: Optional[torch.Tensor] = None, b_mn: bool = False, block_n: int = 0) -> torch.Tensor:
-        """x [M, K_local] bf16, w [N, K_local] (or [K_local, N] with b_mn); bias fp32 [N]; residual bf16 [M, N] (replicated:
-        only this rank's row block is read).  Returns the [M, N] view of `out` (valid after the second barrier, which is
-        enqueued here)."""
-        buf = self.slots[self.turn]
-        self.turn ^= 1
-        lib = buf.lib
-        _peer_sig(lib)
-        M, K = x.shape
-        s = torch.cuda.current_stream().cuda_stream
-        rc = lib.tepd_gemm_bf16_peer(3, (ctypes.c_void_p * self.world)(*([x.data_ptr()] * self.world)), w.data_ptr(), None,
-                                     buf.ptr_array, None, M, self.N, K, x.stride(0), w.stride(0), self.N, int(b_mn), 0,
-                                     self.world, self.rank, block_n, ops._sms(), s, None, None)
-        if rc:
-            raise RuntimeError(f"gemm_all_reduce: GEMM failed ({rc})")
-        ops._count()
-        self.barrier()          # every peer's partial rows for my block have landed in my slots
-        res_ptr = None
-        if residual is not None:
-            assert residual.is_contiguous() and residual.dtype == torch.bfloat16
-            res_ptr = residual.data_ptr() + self.rank * self.rows * self.N * 2
-        rc = lib.tepd_slot_reduce_bcast(buf.local_ptr, self.world, self.rows, self.N, None if bias is None else bias.data_ptr(),
-                                        res_ptr, out.ptr_array, self.rank, 0, s)
-        if rc:
-            raise RuntimeError(f"gemm_all_reduce: slot_reduce failed ({rc})")
-        ops._count()
-        self.barrier()          # every rank's row block is in everybody's output
-        return out.tensor(torch.bfloat16, self.M * self.N).view(self.M, self.N)
-
-
+# ------------------------------------------------------------------------------------------------ tensor-parallel fused GEMM
 class GemmAllReduceMC:
     """Row-parallel linear + ALL-reduce over NVLS: the wgmma GEMM writes its bf16 partial [M, N] straight into a
     symmetric buffer (no staging copy), then ONE multimem kernel reduces it inside the NVSwitch -- every rank pulls its 1/n
     slice with `multimem.ld_reduce` (fp32 accumulation in the switch), adds bias + residual and publishes the finished
     rows to all ranks with `multimem.st`; the two cross-rank barriers live inside that kernel (one `multimem.red` per CTA).
     Per element the owner receives 1x (not (n-1)x) and sends 1x (not (n-1)x): the NVLink bytes of a tensor-parallel
-    all-reduce no longer grow with n.  Same call interface as GemmAllReduce (the unicast slot version)."""
+    all-reduce no longer grow with n.  One instance serves every call site of a given [M, N]; each call site owns its
+    symmetric output buffer, allocated with `new_output()`."""
 
     def __init__(self, M: int, N: int, group=None, ctx: Optional["McContext"] = None, ctas: int = 0):
         self.M, self.N, self.group = M, N, group
@@ -543,64 +395,3 @@ class GemmAllReduceMC:
             assert residual.is_contiguous() and residual.dtype == torch.bfloat16
         self.ctx.all_reduce_bf16_(out, self.M * self.N, self.N, bias=bias, residual=residual, ctas=self.ctas)
         return y
-
-
-class AllGatherGemm:
-    """Column-parallel linear fused with the all-gather of its row-sharded input.  A small copy kernel on a side stream
-    pulls the peers' shards into a local staging buffer chunk by chunk (p2p_gather_chunks) while the persistent GEMM
-    (peer mode 4) starts on the local shard at once and waits, per chunk, on the flag the copy kernel publishes -- the
-    NVLink transfer hides under the tensor-core work of the previous chunk."""
-
-    def __init__(self, rows_per_rank: int, K: int, group=None, barrier: Optional[SymmBarrier] = None, copy_ctas: int = 32):
-        self.rows, self.K = rows_per_rank, K
-        self.world = dist.get_world_size(group)
-        self.rank = dist.get_rank(group)
-        # two shard buffers alternate: a peer may still be copying round i's shard while round i+1's is being produced
-        self.shards = [SymmetricBuffer(rows_per_rank * K * 2, group) for _ in range(2)]
-        self.turn = 0
-        self.barrier = barrier or SymmBarrier(group)
-        dev = torch.device("cuda", torch.cuda.current_device())
-        self.full = torch.empty(rows_per_rank * self.world, K, dtype=torch.bfloat16, device=dev)
-        self.flags = torch.zeros(16, dtype=torch.int32, device=dev)       # [0:8] ready flags, [8:16] arrival counters
-        self.side = torch.cuda.Stream()
-        self.copy_ctas = copy_ctas
-        self._ev0, self._ev1 = torch.cuda.Event(), torch.cuda.Event()
-
-    def input(self) -> torch.Tensor:
-        """The local shard [rows_per_rank, K] (bf16) the producer of the activation writes into before the next call."""
-        return self.shards[self.turn].tensor(torch.bfloat16, self.rows * self.K).view(self.rows, self.K)
-
-    def __call__(self, w: torch.Tensor, bias: Optional[torch.Tensor] = None, out_dtype: torch.dtype = torch.bfloat16,
-                 b_mn: bool = False, block_n: int = 0) -> torch.Tensor:
-        shard = self.shards[self.turn]
-        self.turn ^= 1
-        lib = shard.lib
-        _peer_sig(lib)
-        n = self.world
-        M = self.rows * n
-        N = w.shape[1] if b_mn else w.shape[0]
-        main = torch.cuda.current_stream()
-        self.barrier()                      # every rank's shard is written (and last round's staging reads are done)
-        if n > 1:
-            self._ev0.record(main)
-            self.side.wait_event(self._ev0)
-            rc = lib.tepd_p2p_gather_chunks(shard.ptr_array, self.full.data_ptr(), n, self.rank, self.rows * self.K * 2,
-                                            self.flags.data_ptr(), self.flags.data_ptr() + 32, self.barrier.epoch.data_ptr(),
-                                            self.copy_ctas, self.side.cuda_stream)
-            if rc:
-                raise RuntimeError(f"p2p_gather_chunks failed ({rc})")
-            ops._count()
-        d = torch.empty(M, N, dtype=out_dtype, device=w.device)
-        a_ptrs = [self.full.data_ptr()] * n
-        a_ptrs[self.rank] = shard.local_ptr
-        rc = lib.tepd_gemm_bf16_peer(4, (ctypes.c_void_p * n)(*a_ptrs), w.data_ptr(), d.data_ptr(),
-                                     (ctypes.c_void_p * n)(*([None] * n)), None if bias is None else bias.data_ptr(), M, N,
-                                     self.K, self.K, w.stride(0), N, int(b_mn), int(out_dtype == torch.float32), n, self.rank,
-                                     block_n, ops._sms(), main.cuda_stream, self.flags.data_ptr(), self.barrier.epoch.data_ptr())
-        if rc:
-            raise RuntimeError(f"all_gather_gemm(staged) failed ({rc})")
-        ops._count()
-        if n > 1:
-            self._ev1.record(self.side)
-            main.wait_event(self._ev1)
-        return d

@@ -28,9 +28,9 @@ from ..utils.init import init_tensor
 # fused) instead of GEMM + NCCL + separate adds.  Default in comm = "fused" mode; TEPDIST_TP_FUSED=0 or comm = "nccl" selects
 # the library collectives.
 TP_FUSED = os.environ.get("TEPDIST_TP_FUSED", "1") == "1"
-# test hook: a factory (M, N, group, barrier) -> object with new_output() / __call__(x, w, out, bias, residual, b_mn) that
-# stands in for parallel.symm.GemmAllReduce, so the executor-side chain fusion can be exercised on CPU (gloo) where the
-# peer-memory kernels cannot run
+# test hook: a factory (M, N, group, ctx) -> object with new_output() / __call__(x, w, out, bias, residual, b_mn) that
+# stands in for parallel.symm.GemmAllReduceMC, so the executor-side chain fusion can be exercised on CPU (gloo) where the
+# multimem kernels cannot run (ctx is passed as None)
 TP_FUSED_IMPL = None
 # GPT-MoE: dispatch / combine einsums whose mask comes from moe_dispatch_mask run as route-table row gathers (ops.moe_*), not as
 # dense [G,S,E*C] x [G,S,M] GEMMs; TEPDIST_MOE_SPARSE=0 keeps the dense einsums (the comparator)
@@ -1152,7 +1152,7 @@ class Executor:
         return found
 
     def _plan_tp_fusion(self) -> None:
-        """Execute every chain found by find_tp_chains as ONE GemmAllReduce call at LIN; the downstream nodes of the chain
+        """Execute every chain found by find_tp_chains as ONE GemmAllReduceMC call at LIN; the downstream nodes of the chain
         alias its result."""
         if self.dry_comm:
             return
@@ -1160,34 +1160,25 @@ class Executor:
         self.tp_fuse = self.find_tp_chains(self.g, set(self.gelu_dual) | set(self.gelu_bwd_fuse) | set(self.alias_of))
         if not self.tp_fuse:
             return
-        if TP_FUSED_IMPL is not None:
-            GemmAllReduce, SymmBarrier = TP_FUSED_IMPL, (lambda pg: None)
-        else:
-            from ..parallel.symm import GemmAllReduce, GemmAllReduceMC, McContext, SymmBarrier, symm_backend
+        if TP_FUSED_IMPL is None:
+            from ..parallel.symm import GemmAllReduceMC, McContext, symm_backend
         self._tp_ops: Dict[Tuple[int, int, int], Any] = {}
-        bar: Dict[int, Any] = {}
+        ctx: Dict[int, Any] = {}
         for lid, info in list(self.tp_fuse.items()):
             key = (info["level"], info["M"], info["N"])
-            if TP_FUSED_IMPL is None and key not in self._tp_ops:
-                # without a multicast-bound group (no NVSwitch multicast / IPC fallback) the chain stays on NCCL: the unicast slot
-                # variant (GemmAllReduce) is kept for experiments only (TEPDIST_TP_UNICAST=1), it has not beaten NCCL + cuBLAS
-                pg0 = mesh.group(info["level"])
-                mc_ok = (os.environ.get("TEPDIST_TP_MC", "1") == "1" and symm_backend(pg0) == "vmm"
-                         and (info["M"] * info["N"]) % (8 * info["num"]) == 0)
-                if not mc_ok and os.environ.get("TEPDIST_TP_UNICAST", "0") != "1":
-                    del self.tp_fuse[lid]
-                    continue
             if key not in self._tp_ops:
                 pg = mesh.group(info["level"])
-                # NVLS (multicast) version when the group's symmetric memory is multicast-bound; unicast slots otherwise
-                use_mc = (TP_FUSED_IMPL is None and os.environ.get("TEPDIST_TP_MC", "1") == "1" and symm_backend(pg) == "vmm"
-                          and (info["M"] * info["N"]) % (8 * info["num"]) == 0)
-                if info["level"] not in bar:
-                    bar[info["level"]] = McContext(pg) if use_mc else SymmBarrier(pg)
-                if use_mc:
-                    self._tp_ops[key] = GemmAllReduceMC(info["M"], info["N"], pg, bar[info["level"]])
+                if TP_FUSED_IMPL is not None:
+                    self._tp_ops[key] = TP_FUSED_IMPL(info["M"], info["N"], pg, None)
+                elif symm_backend(pg) == "vmm" and (info["M"] * info["N"]) % (8 * info["num"]) == 0:
+                    if info["level"] not in ctx:
+                        ctx[info["level"]] = McContext(pg)
+                    self._tp_ops[key] = GemmAllReduceMC(info["M"], info["N"], pg, ctx[info["level"]])
                 else:
-                    self._tp_ops[key] = GemmAllReduce(info["M"], info["N"], pg, bar[info["level"]])
+                    # no multicast-bound symmetric memory in this group (no NVSwitch multicast, or the IPC fallback): the
+                    # chain stays on NCCL
+                    del self.tp_fuse[lid]
+                    continue
             info["op"] = self._tp_ops[key]
             info["out"] = info["op"].new_output()        # symmetric [M, N] bf16, written by every rank
             # each chain node aliases its immediate predecessor (lin -> ar -> +bias -> +res): that is the dataflow the

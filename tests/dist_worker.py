@@ -158,12 +158,12 @@ def case_fullstate(strategy):
 
 
 class _EmulatedGemmAllReduce:
-    """CPU stand-in for parallel.symm.GemmAllReduce with the same call contract: row-parallel partial GEMM, sum over the
+    """CPU stand-in for parallel.symm.GemmAllReduceMC with the same call contract: row-parallel partial GEMM, sum over the
     group, + bias + residual.  Lets the EXECUTOR side of the fused tensor-parallel path (chain detection, aliasing of the
-    all_reduce / add nodes, bias / residual plumbing, liveness) run under gloo; the peer-memory kernels are not involved."""
+    all_reduce / add nodes, bias / residual plumbing, liveness) run under gloo; the multimem kernels are not involved."""
     calls = 0
 
-    def __init__(self, M, N, group, barrier):
+    def __init__(self, M, N, group, ctx):
         self.M, self.N, self.group = M, N, group
 
     def new_output(self):

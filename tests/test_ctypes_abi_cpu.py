@@ -1,5 +1,5 @@
 """The Python side talks to the CUDA library through hand-written ctypes argtypes tables (ops/__init__.py `_Sig`,
-parallel/symm.py `_sigs` / `_peer_sig`, parallel/moe.py `_sig`).  A mismatch in COUNT or KIND against the `extern "C"`
+parallel/symm.py `_sigs` / `_vmm_sigs`, parallel/moe.py `_sig`).  A mismatch in COUNT or KIND against the `extern "C"`
 declaration does not fail loudly -- arguments are just reinterpreted.  This test parses every `extern "C" int tepd_*(...)`
 in ops/csrc/*.cu and compares it parameter by parameter with what the Python modules install.  Static check only: it says
 nothing about whether the VALUES passed at the call sites are the right ones."""
@@ -80,7 +80,6 @@ def _python_tables():
     lib = _FakeLib()
     symm._sigs(lib)
     symm._vmm_sigs(lib)
-    symm._peer_sig(lib)
     moe._sig(lib)
     for name, fn in lib.fns.items():
         assert name not in tables, f"{name} has two argtypes tables"

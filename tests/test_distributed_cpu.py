@@ -443,9 +443,9 @@ def test_state_dict_is_whole_and_identical_on_every_rank(tmp_path):
 
 def test_executor_side_of_fused_tp_all_reduce_with_emulated_kernel(tmp_path):
     """The executor's fusion of `linear -> all_reduce [-> + bias] [-> + residual]` chains (TEPDIST_TP_FUSED) with an EMULATED
-    GemmAllReduce (matmul + gloo all-reduce): chain aliasing, bias / residual plumbing and liveness must reproduce the
-    single-process losses.  This validates the executor logic only -- the CUDA kernels behind the real GemmAllReduce
-    (peer-mode-3 GEMM + slot_reduce with broadcast) have still never been executed."""
+    GemmAllReduceMC (matmul + gloo all-reduce): chain aliasing, bias / residual plumbing and liveness must reproduce the
+    single-process losses.  This validates the executor logic only -- the CUDA kernels behind the real GemmAllReduceMC
+    (GEMM into a multicast-bound buffer + the multimem all-reduce) are checked by the multi-GPU tests."""
     ref = _single("gpt2:auto")
     got = _run("tpfused:tp", 2, tmp_path)
     assert got["parallelism"].startswith("tp") and got["fused_calls"] > 0, got

@@ -295,7 +295,7 @@ def test_profile_and_plan_artifact_dumps(tmp_path):
 def test_tp_all_reduce_chains_are_found_for_fusion():
     """Megatron plan of GPT-2: every row-parallel projection is linear -> all_reduce -> +bias -> +residual, every
     column-parallel input gradient is linear_dgrad -> all_reduce; these are the chains the fused GEMM -> all-reduce path
-    (parallel/symm.py GemmAllReduce, TEPDIST_TP_FUSED=1) takes over."""
+    (parallel/symm.py GemmAllReduceMC, TEPDIST_TP_FUSED=1) takes over."""
     from tepdist_b200.models.gpt2 import CONFIGS, build_gpt2_graph
     from tepdist_b200.parallel import plan_spmd
     from tepdist_b200.runtime.executor import Executor

@@ -1,5 +1,5 @@
 """2+ GPU worker: tensor-parallel plan of GPT-2 executed (a) with NCCL collectives and (b) with the fused GEMM -> all-reduce
-path (TEPDIST_TP_FUSED=1, parallel/symm.py GemmAllReduce) -- loss trajectories must agree with each other and with one GPU."""
+path (TEPDIST_TP_FUSED=1, parallel/symm.py GemmAllReduceMC) -- loss trajectories must agree with each other and with one GPU."""
 import json
 import os
 import sys
