@@ -194,6 +194,11 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
 
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     assert a3.stride(2) == 1 and b3.stride(2) == 1 and out3.stride(2) == 1
+    # the epilogue addresses aux (read) and out2 (written) with out's offsets: any other layout reads or writes wrong elements
+    for name, t in (("aux", aux), ("out2", out2)):
+        if t is not None and (t.dtype != torch.bfloat16 or t.shape != out.shape or t.stride() != out.stride()):
+            raise ValueError(f"gemm: {name} must be bf16 with out's shape {tuple(out.shape)} and strides {out.stride()}; "
+                             f"got {t.dtype} {tuple(t.shape)} strides {t.stride()}")
     if STREAM_K_FWD and split_k == 0 and block_n == 0 and not batched and not accumulate and K >= 512:
         # wave quantisation check for the persistent 128x256 schedule: below ~93 % SM occupancy the stream-K schedule
         # (equal k-block ranges per SM + workspace fix-up of split tiles) wins over both tile-parallel kernels
