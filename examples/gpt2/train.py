@@ -30,11 +30,16 @@ def main():
     ap.add_argument("--data", default=None, help="comma-separated token files (see tepdist_b200.data.write_token_file) or 'synthetic'")
     ap.add_argument("--data-int32", action="store_true", help="token files hold int32 ids (default uint16)")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--eot-token", type=int, default=None,
+                    help="end-of-text token id (50256 for GPT-2): attention stays inside each packed document")
+    ap.add_argument("--reset-position-ids", action="store_true",
+                    help="learned positions count from each document's start (needs --eot-token)")
     a = ap.parse_args()
     clip = {"clip_norm": a.clip_norm, "clip_norm_value": a.clip_norm_value} if a.clip_norm else {}
     cfg = CONFIGS[a.model]
     world = int(os.environ.get("WORLD_SIZE", "1"))
-    g = build_gpt2_graph(cfg, batch=a.batch * world, optimizer=a.optimizer, **clip)
+    g = build_gpt2_graph(cfg, batch=a.batch * world, optimizer=a.optimizer, eot_token=a.eot_token,
+                         reset_position_ids=a.reset_position_ids, **clip)
     tr = Trainer(g, strategy=a.strategy, comm_mode=a.comm)
     if a.warmup_steps > 0:
         from tepdist_b200.utils.schedules import warmup_cosine

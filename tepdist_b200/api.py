@@ -56,6 +56,8 @@ class Trainer:
         self._fake_feeds: Optional[Dict[str, torch.Tensor]] = None
         grad_sync = None
         self.plan_info: Dict[str, Any] = {"strategy": strategy, "world": self.world}
+        from .parallel import check_context_parallel
+        check_context_parallel(graph, config.resolve_strategy(strategy))
         from .planner import liveness_optimize
         graph, copies = liveness_optimize(graph)    # per-user copies of large convert(variable) results (B6)
         if copies:

@@ -204,8 +204,23 @@ void LayerNormBwdRule(Ctx& c) {
 // merge by log-sum-exp.  The reference has no such op (SURVEY 5.7: long context = token split + what XLA SPMD makes of the dots);
 // priced as the K / V all-gather it replaces (forward) plus the dK / dV reduce-scatter (backward).
 double RingBytes(const TensorType& qkv, int num) { return (double)qkv.bytes() * (2.0 / 3.0) * (num - 1) / num; }
+// Document-masked attention (a 2nd input doc_start [B,S]; attention_bwd: a 5th) has no "seq" candidate: the ring does not carry
+// document starts, so context parallelism with document masks is not offered.  It splits over the batch (doc_start with it)
+// or over heads (doc_start replicated).
+void DocAttentionRule(Ctx& c, int qkv_idx) {
+  const int64_t H = c.n.attr_i("heads");
+  const int nin = c.nin();
+  std::vector<DS> batch(nin, c.S(0)), heads(nin, c.S(2));
+  heads[nin - 1] = c.G();
+  if (c.n.op == "attention_bwd") heads[3] = c.S(1);   // lse [B,H,S]
+  if (c.divisible(c.in(qkv_idx), 0))
+    c.add(batch, c.n.op == "attention" ? std::vector<DS>{c.S(0), c.S(0)} : std::vector<DS>{c.S(0)}, "batch");
+  if (H % c.num == 0) c.add(heads, c.n.op == "attention" ? std::vector<DS>{c.S(2), c.S(1)} : std::vector<DS>{c.S(2)}, "heads");
+  c.add_glue();
+}
 void AttentionRule(Ctx& c, const RuleOptions& opt) {
   // qkv [B,S,H*3*D] (heads-major, so a plain last-dim split is a split over heads) -> o [B,S,H*D], lse [B,H,S]
+  if (c.nin() == 2) return DocAttentionRule(c, 0);
   const int64_t H = c.n.attr_i("heads");
   const bool cp = opt.context_parallel && c.divisible(c.in(0), 1);   // "cp": the sequence split is the only way through attention
   if (c.divisible(c.in(0), 0) && !cp) c.add({c.S(0)}, {c.S(0), c.S(0)}, "batch");
@@ -214,6 +229,7 @@ void AttentionRule(Ctx& c, const RuleOptions& opt) {
   if (!cp) c.add_glue();   // (replicated attention = n x the S^2 FLOPs per rank: never what "cp" asks for)
 }
 void AttentionBwdRule(Ctx& c, const RuleOptions& opt) {
+  if (c.nin() == 5) return DocAttentionRule(c, 1);
   const int64_t H = c.n.attr_i("heads");  // (do, qkv, o, lse) -> dqkv
   const bool cp = opt.context_parallel && c.divisible(c.in(1), 1);
   if (c.divisible(c.in(1), 0) && !cp) c.add({c.S(0), c.S(0), c.S(0), c.S(0)}, {c.S(0)}, "batch");
@@ -221,14 +237,26 @@ void AttentionBwdRule(Ctx& c, const RuleOptions& opt) {
   if (c.divisible(c.in(1), 1)) c.add({c.S(1), c.S(1), c.S(1), c.S(2)}, {c.S(1)}, "seq", 2.0 * RingBytes(c.in(1), c.num));
   if (!cp) c.add_glue();
 }
-void EmbeddingRule(Ctx& c) {  // tokens[B,S], wte[V,C], wpe[S,C] -> [B,S,C]
+void EmbeddingRule(Ctx& c) {  // tokens[B,S], wte[V,C], wpe[S,C] (, doc_start[B,S]) -> [B,S,C]
+  if (c.nin() == 4) {   // per-document positions: any row of wpe can be read anywhere, so it stays whole (no "seq")
+    if (c.divisible(c.in(0), 0)) c.add({c.S(0), c.G(), c.G(), c.S(0)}, {c.S(0)}, "batch");
+    c.add({c.G(), c.S(1), c.S(1), c.G()}, {c.S(2)}, "hidden");
+    c.add_glue();
+    return;
+  }
   if (c.divisible(c.in(0), 0)) c.add({c.S(0), c.G(), c.G()}, {c.S(0)}, "batch");
   // sequence split: rank r embeds positions [r S/n, (r+1) S/n) -- exactly the rows of a position table stored split on dim 0
   if (c.divisible(c.in(0), 1) && c.in(2).dims[0] == c.in(0).dims[1]) c.add({c.S(1), c.G(), c.S(0)}, {c.S(1)}, "seq");
   c.add({c.G(), c.S(1), c.S(1)}, {c.S(2)}, "hidden");
   c.add_glue();
 }
-void EmbeddingBwdRule(Ctx& c) {  // tokens, dy[B,S,C] -> dwte[V,C], dwpe[S,C]
+void EmbeddingBwdRule(Ctx& c) {  // tokens, dy[B,S,C] (, doc_start[B,S]) -> dwte[V,C], dwpe[S,C]
+  if (c.nin() == 3) {
+    if (c.divisible(c.in(0), 0)) c.add({c.S(0), c.S(0), c.S(0)}, {c.P(), c.P()}, "batch");
+    c.add({c.G(), c.S(2), c.G()}, {c.S(1), c.S(1)}, "hidden");
+    c.add_glue();
+    return;
+  }
   if (c.divisible(c.in(0), 0)) c.add({c.S(0), c.S(0)}, {c.P(), c.P()}, "batch");
   if (c.divisible(c.in(0), 1) && c.o(1).dims[0] == c.in(0).dims[1]) c.add({c.S(1), c.S(1)}, {c.P(), c.S(0)}, "seq");
   c.add({c.G(), c.S(2)}, {c.S(1), c.S(1)}, "hidden");
@@ -514,6 +542,10 @@ std::vector<Candidate> EnumerateCandidates(const Graph& g, const Node& n, int nu
   else if (op == "attention_bwd") AttentionBwdRule(c, opt);
   else if (op == "embedding") EmbeddingRule(c);
   else if (op == "embedding_bwd") EmbeddingBwdRule(c);
+  else if (op == "doc_starts") {   // a running max along each row: a sequence split would cut it
+    if (c.divisible(c.in(0), 0)) c.add({c.S(0)}, {c.S(0)}, "batch");
+    c.add_glue();
+  }
   else if (op == "softmax_xent") XentRule(c);
   else if (op == "colsum") ColsumRule(c);
   else if (op == "reduce_sum" || op == "reduce_mean" || op == "reduce_max") ReduceRule(c);

@@ -58,10 +58,17 @@ class GraphBuilder:
         return self._n("constant", [], [TensorType(tuple(shape), dtype)], {"value": value}).out()
 
     # ------------------------------------------------------------------ macro ops (map 1:1 onto sm_90a kernels)
-    def embedding(self, tokens: Value, wte: Value, wpe: Value, name="embed") -> Value:
+    def embedding(self, tokens: Value, wte: Value, wpe: Value, doc_starts: Optional[Value] = None, name="embed") -> Value:
+        """wte[tokens] + wpe[position]; with `doc_starts` (see `doc_starts`) the position counts from the token's document
+        start (per-document positions)."""
         B, S = self.t(tokens).shape
         C = self.t(wte).shape[1]
-        return self._n("embedding", [tokens, wte, wpe], [TensorType((B, S, C), self.t(wte).dtype)], {}, name).out()
+        ins = [tokens, wte, wpe] + ([doc_starts] if doc_starts is not None else [])
+        return self._n("embedding", ins, [TensorType((B, S, C), self.t(wte).dtype)], {}, name).out()
+
+    def doc_starts(self, tokens: Value, eot: int, name="doc_starts") -> Value:
+        """i32 [B, S]: 1 + the position of the last end-of-text token `eot` before s in its row, or 0 (packed documents)."""
+        return self._n("doc_starts", [tokens], [TensorType(tuple(self.t(tokens).shape), "i32")], {"eot": int(eot)}, name).out()
 
     def layernorm(self, x: Value, gamma: Value, beta: Value, eps: float = 1e-5, name="ln") -> Value:
         return self._n("layernorm", [x, gamma, beta], [self.t(x)], {"eps": eps}, name).out()
@@ -82,10 +89,16 @@ class GraphBuilder:
     def gelu(self, x: Value, name="gelu") -> Value:
         return self._n("gelu", [x], [self.t(x)], {}, name).out()
 
-    def attention(self, qkv: Value, heads: int, causal: bool = True, name="attn") -> Value:
+    def attention(self, qkv: Value, heads: int, causal: bool = True, doc_starts: Optional[Value] = None,
+                  name="attn") -> Value:
+        """Fused attention over qkv [B, S, 3C] (heads-major).  `doc_starts` (causal only) restricts every query to the keys
+        of its own document."""
         B, S, C3 = self.t(qkv).shape
         C = C3 // 3
-        n = self._n("attention", [qkv], [TensorType((B, S, C), self.t(qkv).dtype), TensorType((B, heads, S), "f32")],
+        if doc_starts is not None and not causal:
+            raise ValueError("attention: document masking (doc_starts) is defined for causal attention only")
+        ins = [qkv] + ([doc_starts] if doc_starts is not None else [])
+        n = self._n("attention", ins, [TensorType((B, S, C), self.t(qkv).dtype), TensorType((B, heads, S), "f32")],
                     {"heads": heads, "causal": causal}, name)
         return n.out(0)
 
@@ -344,10 +357,12 @@ def backward(b: GraphBuilder, loss: Value) -> Dict[int, Value]:
             push(n.inputs[0], B("gelu_bwd", [dy, n.inputs[0]], [T(n.inputs[0])], {}, grp).out())
         elif n.op == "attention":
             qkv = n.inputs[0]
-            push(qkv, B("attention_bwd", [dy, qkv, Value(n.id, 0), Value(n.id, 1)], [T(qkv)], dict(n.attrs), grp).out())
+            push(qkv, B("attention_bwd", [dy, qkv, Value(n.id, 0), Value(n.id, 1)] + n.inputs[1:], [T(qkv)], dict(n.attrs),
+                        grp).out())
         elif n.op == "embedding":
-            tok, wte, wpe = n.inputs
-            nb = B("embedding_bwd", [tok, dy], [TensorType(T(wte).shape, "f32"), TensorType(T(wpe).shape, "f32")], {}, grp)
+            tok, wte, wpe = n.inputs[:3]
+            nb = B("embedding_bwd", [tok, dy] + n.inputs[3:], [TensorType(T(wte).shape, "f32"), TensorType(T(wpe).shape, "f32")],
+                   {}, grp)
             push(wte, nb.out(0)); push(wpe, nb.out(1))
         elif n.op in ("add", "sub"):
             x, y = n.inputs

@@ -54,7 +54,13 @@ CONFIGS = {
 }
 
 
-def build_gpt2_graph(cfg: GPT2Config, batch: int | None = None, optimizer: str = "adamw", **opt_hp) -> Graph:
+def build_gpt2_graph(cfg: GPT2Config, batch: int | None = None, optimizer: str = "adamw", eot_token: int | None = None,
+                     reset_position_ids: bool = False, **opt_hp) -> Graph:
+    """`eot_token`: rows are packed documents separated by this token; every attention layer then masks attention to the
+    query's own document (one `doc_starts` node feeds all of them).  `reset_position_ids` (needs `eot_token`): learned
+    positions count from each document's start."""
+    if reset_position_ids and eot_token is None:
+        raise ValueError("reset_position_ids needs eot_token (the documents come from its positions)")
     B = batch or cfg.batch
     S, C, H, V, Vp = cfg.n_ctx, cfg.n_embd, cfg.n_head, cfg.n_vocab, cfg.padded_vocab
     b = GraphBuilder(cfg.name)
@@ -65,14 +71,15 @@ def build_gpt2_graph(cfg: GPT2Config, batch: int | None = None, optimizer: str =
     with b.scope("model"):
         wte = b.parameter("wte", (Vp, C), nrm(0.02))
         wpe = b.parameter("wpe", (S, C), nrm(0.01))
-        x = b.embedding(tokens, wte, wpe)
+        ds = b.doc_starts(tokens, eot_token) if eot_token is not None else None
+        x = b.embedding(tokens, wte, wpe, doc_starts=ds if reset_position_ids else None)
         for l in range(cfg.n_layer):
             with b.scope(f"h{l}"):
                 g1 = b.parameter("ln_1/g", (C,), const(1.0)); b1 = b.parameter("ln_1/b", (C,), const(0.0))
                 h = b.layernorm(x, g1, b1, name="ln_1")
                 w_qkv = b.parameter("attn/c_attn/w", (3 * C, C), nrm(0.02)); b_qkv = b.parameter("attn/c_attn/b", (3 * C,), const(0.0))
                 qkv = b.linear(h, w_qkv, b_qkv, name="attn/c_attn")
-                a = b.attention(qkv, heads=H, causal=True, name="attn/core")
+                a = b.attention(qkv, heads=H, causal=True, doc_starts=ds, name="attn/core")
                 w_o = b.parameter("attn/c_proj/w", (C, C), nrm(0.02 / math.sqrt(2 * cfg.n_layer))); b_o = b.parameter("attn/c_proj/b", (C,), const(0.0))
                 x = b.linear(a, w_o, b_o, residual=x, name="attn/c_proj")
                 g2 = b.parameter("ln_2/g", (C,), const(1.0)); b2 = b.parameter("ln_2/b", (C,), const(0.0))
@@ -90,5 +97,5 @@ def build_gpt2_graph(cfg: GPT2Config, batch: int | None = None, optimizer: str =
     g = build_training_step(b, loss, optimizer, **{**dict(lr=cfg.lr, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=cfg.weight_decay),
                                                      **opt_hp})      # (opt_hp: clip_norm / clip_norm_value / schedule / ...)
     g.meta["model"] = {"family": "gpt2", "name": cfg.name, "n_layer": cfg.n_layer, "n_embd": C, "n_head": H,
-                       "n_ctx": S, "n_vocab": V, "batch": B}
+                       "n_ctx": S, "n_vocab": V, "batch": B, "eot_token": eot_token, "reset_position_ids": bool(reset_position_ids)}
     return g

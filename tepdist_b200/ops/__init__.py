@@ -89,8 +89,9 @@ class _Sig:
     tepd_bn_bwd_apply_nhwc = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp]
     tepd_im2col_nhwc = [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]
     tepd_col2im_nhwc = [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]
-    tepd_embedding_fwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]
-    tepd_embedding_bwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]
+    tepd_embedding_fwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]
+    tepd_embedding_bwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]
+    tepd_doc_starts = [_vp, _vp, _i, _i, _i, _vp]
     tepd_xent_fwd_bwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp]
     tepd_adamw = [_vp, _vp, _vp, _vp, _vp, _ll, _ll, _f, _f, _f, _f, _f, _f, _f, _f, _vp, _vp]
     tepd_sgd = [_vp, _vp, _vp, _ll, _f, _f, _vp]
@@ -106,9 +107,9 @@ class _Sig:
     tepd_gap_bwd_nhwc = [_vp, _vp, _i, _i, _i, _vp]
     tepd_attn_merge = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]
     tepd_attn_ring_accum = [_vp, _vp, _vp, _ll, _i, _i, _vp]
-    tepd_attn_fwd = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _ll, _ll, _ll, _vp]
+    tepd_attn_fwd = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _ll, _ll, _ll, _vp, _vp]
     tepd_attn_bwd = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i,
-                     _ll, _ll, _ll, _ll, _ll, _ll, _vp]
+                     _ll, _ll, _ll, _ll, _ll, _ll, _vp, _vp]
 
 
 def _stream() -> int:
@@ -693,33 +694,70 @@ def colsum_acc(x: torch.Tensor, out_acc: torch.Tensor) -> None:
     _count()
 
 
-# --------------------------------------------------------------------------------------------- embedding
-def embedding_fwd(tokens: torch.Tensor, wte: torch.Tensor, wpe: torch.Tensor) -> torch.Tensor:
+# --------------------------------------------------------------------------------------------- documents
+def doc_starts(tokens: torch.Tensor, eot: int) -> torch.Tensor:
+    """int32 [B, S]: doc_start[b, s] = 1 + the last p < s with tokens[b, p] == eot, or 0 (the end-of-text token belongs to
+    the document it ends; a row that begins inside a document treats that part as its first document)."""
     B, S = tokens.shape
-    C = wte.shape[1]
     if not tokens.is_cuda:
-        pos = torch.arange(S, device=tokens.device)
-        return (wte[tokens.long()].float() + wpe[pos].float()).to(wte.dtype)
-    out = torch.empty(B, S, C, dtype=wte.dtype, device=wte.device)
+        pos = torch.arange(1, S + 1, device=tokens.device).expand(B, S)
+        run = torch.where(tokens.long() == eot, pos, 0).cummax(1).values   # 1 + the last EOT at or before s
+        out = torch.zeros(B, S, dtype=torch.int32, device=tokens.device)
+        out[:, 1:] = run[:, :-1]
+        return out
     tok = tokens.to(torch.int32).contiguous()
-    _check(lib().tepd_embedding_fwd(tok.data_ptr(), wte.data_ptr(), wpe.data_ptr(), out.data_ptr(), B * S, S, C,
-                                    _stream()), "embedding_fwd")
+    out = torch.empty(B, S, dtype=torch.int32, device=tokens.device)
+    _check(lib().tepd_doc_starts(tok.data_ptr(), out.data_ptr(), B, S, int(eot), _stream()), "doc_starts")
     _count()
     return out
 
 
-def embedding_bwd(tokens: torch.Tensor, dout: torch.Tensor, dwte_acc: torch.Tensor, dwpe_acc: torch.Tensor) -> None:
+def _doc_ptr(doc_start: Optional[torch.Tensor], B: int, S: int) -> Optional[torch.Tensor]:
+    """doc_start as the int32 contiguous [B, S] tensor the kernels read (None stays None)."""
+    if doc_start is None:
+        return None
+    assert tuple(doc_start.shape) == (B, S), f"doc_start {tuple(doc_start.shape)} != {(B, S)}"
+    return doc_start.to(torch.int32).contiguous()
+
+
+# --------------------------------------------------------------------------------------------- embedding
+def embedding_fwd(tokens: torch.Tensor, wte: torch.Tensor, wpe: torch.Tensor,
+                  doc_start: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """wte[tokens] + wpe[position]; the position is s, or s - doc_start[b, s] (per-document positions) when given."""
+    B, S = tokens.shape
+    C = wte.shape[1]
+    if not tokens.is_cuda:
+        pos = torch.arange(S, device=tokens.device)
+        if doc_start is not None:
+            pos = pos - doc_start.long()
+        return (wte[tokens.long()].float() + wpe[pos].float()).to(wte.dtype)
+    out = torch.empty(B, S, C, dtype=wte.dtype, device=wte.device)
+    tok = tokens.to(torch.int32).contiguous()
+    ds = _doc_ptr(doc_start, B, S)
+    _check(lib().tepd_embedding_fwd(tok.data_ptr(), wte.data_ptr(), wpe.data_ptr(), out.data_ptr(), B * S, S, C,
+                                    _stream(), _p(ds)), "embedding_fwd")
+    _count()
+    return out
+
+
+def embedding_bwd(tokens: torch.Tensor, dout: torch.Tensor, dwte_acc: torch.Tensor, dwpe_acc: torch.Tensor,
+                  doc_start: Optional[torch.Tensor] = None) -> None:
     B, S = tokens.shape
     C = dout.shape[-1]
     if not tokens.is_cuda:
         d = dout.float().reshape(B * S, C)
         dwte_acc.index_add_(0, tokens.reshape(-1).long(), d)
-        dwpe_acc[:S].add_(dout.float().reshape(B, S, C).sum(0))
+        if doc_start is None:
+            dwpe_acc[:S].add_(dout.float().reshape(B, S, C).sum(0))
+        else:
+            pos = torch.arange(S, device=tokens.device) - doc_start.long()
+            dwpe_acc.index_add_(0, pos.reshape(-1), d)
         return
     tok = tokens.to(torch.int32).contiguous()
     dout = dout.contiguous()
+    ds = _doc_ptr(doc_start, B, S)
     _check(lib().tepd_embedding_bwd(tok.data_ptr(), dout.data_ptr(), dwte_acc.data_ptr(), dwpe_acc.data_ptr(), B * S, S,
-                                    C, _stream()), "embedding_bwd")
+                                    C, _stream(), _p(ds)), "embedding_bwd")
     _count()
 
 

@@ -7,6 +7,9 @@ contiguous [B, S, H, D] tensor, i.e. already the [tokens, hidden] input of the o
 On CUDA tensors the wgmma kernels cover head widths 64 and 128 with S % 128 == 0; narrower heads and a ragged causal
 sequence length are zero-padded onto them (see `_can_pad`).  The remaining shapes (D > 128, non-causal ragged S) run
 plain torch math, which materialises [B, H, S, S] fp32 scores, and warn once per shape.
+
+Document masking (packed rows): with ``doc_start`` (int32 [B, S], non-decreasing along S, see ``ops.doc_starts``) query s
+attends to keys doc_start[b, s] <= k <= s.  It is defined for causal attention only.
 """
 from __future__ import annotations
 
@@ -37,19 +40,42 @@ def _pad_sd(t: torch.Tensor, S: int, D: int, W: int) -> torch.Tensor:
     return torch.nn.functional.pad(t, (0, W - D, 0, 0, 0, Sp - S))
 
 
+def _pad_doc(doc_start: torch.Tensor | None, S: int) -> torch.Tensor | None:
+    """[B, S] -> [B, ceil128(S)] repeating the last document start (keeps it non-decreasing; the padded rows are dropped)."""
+    Sp = (S + 127) // 128 * 128
+    if doc_start is None or Sp == S:
+        return doc_start
+    return torch.cat([doc_start, doc_start[:, -1:].expand(-1, Sp - S)], 1)
+
+
+def _check_doc(doc_start, causal: bool) -> None:
+    if doc_start is not None and not causal:
+        raise ValueError("attention: document masking (doc_start) is defined for causal attention only")
+
+
+def _mask(S: int, causal: bool, doc_start, device):
+    """Boolean mask of the visible (query, key) pairs, broadcastable to [B, H, S, S], or None."""
+    if not causal:
+        return None
+    mask = torch.ones(S, S, dtype=torch.bool, device=device).tril()
+    if doc_start is not None:
+        keys = torch.arange(S, device=device)
+        mask = mask & (keys.view(1, 1, S) >= doc_start.to(device).long().unsqueeze(-1)).unsqueeze(1)   # [B, 1, S, S]
+    return mask
+
+
 def _warn_torch_math(S: int, D: int, causal: bool) -> None:
     from . import _warn_once
     _warn_once(f"attention: no kernel for head dim {D}, seq {S}, causal={causal}; running torch math with "
                f"[B, H, {S}, {S}] fp32 scores")
 
 
-def _ref_fwd(q, k, v, scale, causal):
+def _ref_fwd(q, k, v, scale, causal, doc_start=None):
     # q,k,v: [B,S,H,D] -> fp32 math in [B,H,S,D]
     qf, kf, vf = (t.float().permute(0, 2, 1, 3) for t in (q, k, v))
     s = torch.matmul(qf, kf.transpose(-1, -2)) * scale
-    if causal:
-        S = q.shape[1]
-        mask = torch.ones(S, S, dtype=torch.bool, device=q.device).tril()
+    mask = _mask(q.shape[1], causal, doc_start, q.device)
+    if mask is not None:
         s = s.masked_fill(~mask, float("-inf"))
     lse = torch.logsumexp(s, -1)  # [B,H,S]
     p = torch.exp(s - lse.unsqueeze(-1))
@@ -58,39 +84,42 @@ def _ref_fwd(q, k, v, scale, causal):
 
 
 def attention_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: float | None = None,
-                  causal: bool = True):
-    """Returns (o [B,S,H,D], lse [B,H,S])."""
+                  causal: bool = True, doc_start: torch.Tensor | None = None):
+    """Returns (o [B,S,H,D], lse [B,H,S]).  ``doc_start`` (int32 [B, S]) adds the document mask."""
     B, S, H, D = q.shape
+    _check_doc(doc_start, causal)
     if scale is None:
         scale = 1.0 / math.sqrt(D)
     if not q.is_cuda:
-        o, lse, _ = _ref_fwd(q, k, v, scale, causal)
+        o, lse, _ = _ref_fwd(q, k, v, scale, causal, doc_start)
         return o, lse
     if D not in _KERNEL_WIDTHS or S % 128:
         if _can_pad(S, D, causal):
             W = _kernel_width(D)
             qp, kp, vp = (_pad_sd(t, S, D, W) for t in (q, k, v))
-            o, lse = attention_fwd(qp, kp, vp, scale, causal)
+            o, lse = attention_fwd(qp, kp, vp, scale, causal, _pad_doc(doc_start, S))
             return o[:, :S, :, :D].contiguous(), lse[:, :, :S].contiguous()
         _warn_torch_math(S, D, causal)
-        o, lse, _ = _ref_fwd(q, k, v, scale, causal)   # shapes the wgmma kernels do not cover: plain torch math
+        o, lse, _ = _ref_fwd(q, k, v, scale, causal, doc_start)   # shapes the wgmma kernels do not cover: plain torch math
         return o, lse
-    from . import lib, _check, _count, _stream
+    from . import lib, _check, _count, _stream, _doc_ptr, _p
     assert q.dtype == torch.bfloat16 and q.stride(3) == 1
     assert q.stride() == k.stride() == v.stride(), "q/k/v must share strides (slices of one qkv buffer)"
+    ds = _doc_ptr(doc_start, B, S)
     o = torch.empty(B, S, H, D, dtype=q.dtype, device=q.device)
     lse = torch.empty(B, H, S, dtype=torch.float32, device=q.device)
     _check(lib().tepd_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), B, H, S, D,
-                               float(scale), int(causal), q.stride(0), q.stride(1), q.stride(2), _stream()),
+                               float(scale), int(causal), q.stride(0), q.stride(1), q.stride(2), _stream(), _p(ds)),
            "attn_fwd")
     _count()
     return o, lse
 
 
 def attention_bwd(do: torch.Tensor, q, k, v, o, lse, scale: float | None = None, causal: bool = True,
-                  dqkv_out: torch.Tensor | None = None):
+                  dqkv_out: torch.Tensor | None = None, doc_start: torch.Tensor | None = None):
     """Returns (dq, dk, dv) as [B,S,H,D] views (of ``dqkv_out`` [B,S,H,3,D] when given)."""
     B, S, H, D = q.shape
+    _check_doc(doc_start, causal)
     if scale is None:
         scale = 1.0 / math.sqrt(D)
     if dqkv_out is None:
@@ -100,7 +129,8 @@ def attention_bwd(do: torch.Tensor, q, k, v, o, lse, scale: float | None = None,
         Sp = (S + 127) // 128 * 128
         W = _kernel_width(D)
         lse_p = lse if Sp == S else torch.nn.functional.pad(lse, (0, Sp - S))
-        gq, gk, gv = attention_bwd(*(_pad_sd(t, S, D, W) for t in (do, q, k, v, o)), lse_p, scale, causal)
+        gq, gk, gv = attention_bwd(*(_pad_sd(t, S, D, W) for t in (do, q, k, v, o)), lse_p, scale, causal,
+                                   doc_start=_pad_doc(doc_start, S))
         dq.copy_(gq[:, :S, :, :D]); dk.copy_(gk[:, :S, :, :D]); dv.copy_(gv[:, :S, :, :D])
         return dq, dk, dv
     if not q.is_cuda or D not in _KERNEL_WIDTHS or S % 128:
@@ -111,8 +141,8 @@ def attention_bwd(do: torch.Tensor, q, k, v, o, lse, scale: float | None = None,
         # probabilities from the GIVEN log-sum-exp (like the kernels): a block of a longer key sequence (ring attention) passes
         # the log-sum-exp over ALL keys, and its probabilities must not be re-normalised over the block
         sc = torch.matmul(qf, kf.transpose(-1, -2)) * scale
-        if causal:
-            mask = torch.ones(S, S, dtype=torch.bool, device=q.device).tril()
+        mask = _mask(S, causal, doc_start, q.device)
+        if mask is not None:
             sc = sc.masked_fill(~mask, float("-inf"))
         p = torch.exp(sc - lse.float().unsqueeze(-1))
         dvf = torch.matmul(p.transpose(-1, -2), dof)
@@ -125,14 +155,15 @@ def attention_bwd(do: torch.Tensor, q, k, v, o, lse, scale: float | None = None,
         dk.copy_(dkf.permute(0, 2, 1, 3).to(q.dtype))
         dv.copy_(dvf.permute(0, 2, 1, 3).to(q.dtype))
         return dq, dk, dv
-    from . import lib, _check, _count, _stream
+    from . import lib, _check, _count, _stream, _doc_ptr, _p
     do = do.contiguous()
     assert o.is_contiguous() and do.is_contiguous()
+    ds = _doc_ptr(doc_start, B, S)
     # dq accumulator: persistent self-clearing fp32 workspace inside the library (no per-call memset)
     _check(lib().tepd_attn_bwd(do.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
                                None, dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, H, S, D,
                                float(scale), int(causal), q.stride(0), q.stride(1), q.stride(2),
-                               dq.stride(0), dq.stride(1), dq.stride(2), _stream()), "attn_bwd")
+                               dq.stride(0), dq.stride(1), dq.stride(2), _stream(), _p(ds)), "attn_bwd")
     _count(3)
     return dq, dk, dv
 

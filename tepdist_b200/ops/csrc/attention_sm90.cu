@@ -55,13 +55,17 @@ struct AttnFwdParams {
   int B, H, S, causal;
   float scale_log2;  // softmax scale * log2(e)
   float scale;
+  const int* doc_start;   // int32 [B, S], DOC kernels only: query s sees keys [doc_start[b, s], s]
 };
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-template <int HD>
+// DOC (document-masked causal attention): a query tile starts its KV loop at the tile holding the document start of its
+// first row (doc_start is non-decreasing along the sequence), and tiles below the document start of its last row get an
+// element mask.  A row can then see a fully masked tile, so the softmax subtracts 0 instead of a -inf running max.
+template <int HD, bool DOC>
 __global__ void __launch_bounds__(AttnCfg<HD>::THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const AttnFwdParams p) {
@@ -96,6 +100,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
   __syncthreads();
   pdl_wait();
+  int j0 = 0;   // first KV tile (stage and phase indices count from it)
+  if constexpr (DOC) j0 = __ldg(p.doc_start + (size_t)b * p.S + qi * BQ) / BKV;
 
   if (HD == 64 ? warp == 8 : warp >= 8) {   // producer: warp 8 (D = 64) / warpgroup 2 (D = 128)
     if constexpr (HD == 128) setmaxnreg_dec<24>();
@@ -103,9 +109,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       mbar_expect_tx(q_full, L::TILE_BYTES);
 #pragma unroll
       for (int c = 0; c < NC; ++c) tma_load_4d(smem + L::SM_Q + c * CHUNK, &tmap_q, q_full, c * 64, qi * BQ, h, b);
-      for (int j = 0; j < nkv; ++j) {
-        const int st = j % KV_STAGES;
-        mbar_wait(&kv_empty[st], ((j / KV_STAGES) & 1) ^ 1);
+      for (int j = j0; j < nkv; ++j) {
+        const int st = (j - j0) % KV_STAGES;
+        mbar_wait(&kv_empty[st], (((j - j0) / KV_STAGES) & 1) ^ 1);
         mbar_expect_tx(&kv_full[st], 2 * L::TILE_BYTES);
 #pragma unroll
         for (int c = 0; c < NC; ++c)
@@ -128,10 +134,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  int ds[2] = {0, 0}, ds_last = 0;   // DOC: document starts of this thread's two rows and of the tile's last row
+  if constexpr (DOC) {
+    const int* dsb = p.doc_start + (size_t)b * p.S + qi * BQ;
+    ds[0] = __ldg(dsb + row0);
+    ds[1] = __ldg(dsb + row0 + 8);
+    ds_last = __ldg(dsb + BQ - 1);
+  }
   mbar_wait(q_full, 0);
-  for (int j = 0; j < nkv; ++j) {
-    const int st = j % KV_STAGES;
-    mbar_wait(&kv_full[st], (j / KV_STAGES) & 1);
+  for (int j = j0; j < nkv; ++j) {
+    const int st = (j - j0) % KV_STAGES;
+    mbar_wait(&kv_full[st], ((j - j0) / KV_STAGES) & 1);
     const uint32_t sk = smem_u32(smem + L::SM_K + st * L::TILE_BYTES), sv = smem_u32(smem + L::SM_V + st * L::TILE_BYTES);
     float s[64];
     wgmma_fence();
@@ -143,6 +156,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     wgmma_wait<0>();
     fence_regs(s);
     const bool diag = p.causal && j == qi;
+    if (DOC && j * BKV < ds_last) {   // some key of this tile lies before the document start of some row (a separate pass:
+                                      // the tiles without one run the plain softmax)
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (j * BKV + 8 * jj + 2 * q + (e & 1) < ds[e >> 1]) s[4 * jj + e] = -INFINITY;
+    }
 #pragma unroll
     for (int hr = 0; hr < 2; ++hr) {
       const int r = row0 + hr * 8;
@@ -160,7 +181,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       }
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      const float alpha = exp2f(m[hr] - mx);
+      // safe max: a row that has seen only masked keys keeps m = -inf, and subtracting 0 instead gives p = 0, alpha = 0
+      const float mxs = DOC && mx == -INFINITY ? 0.f : mx;
+      const float alpha = exp2f(m[hr] - mxs);
       m[hr] = mx;
       float sum = 0.f;
 #pragma unroll
@@ -168,7 +191,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int idx = 4 * jj + 2 * hr + e;
-          const float pv = exp2f(s[idx] - mx);
+          const float pv = exp2f(s[idx] - mxs);
           s[idx] = pv;
           sum += pv;
         }
@@ -221,6 +244,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 // =====================================================================================================
 constexpr int BQB = 64;                          // query rows per backward iteration
 
+// The backward's producer is a whole warpgroup that hands its registers to the consumers (setmaxnreg) at D = 128, and also
+// for the document-masked D = 64 kernel, whose extra masking state would otherwise spill under the 288-thread layout.
+template <int HD, bool DOC>
+struct BwdLayout {
+  static constexpr bool WG_PRODUCER = HD == 128 || DOC;
+  static constexpr int THREADS = WG_PRODUCER ? 384 : AttnCfg<HD>::THREADS;
+};
+
 template <int HD>
 struct BwdSmem {
   static constexpr int KV_BYTES = 128 * HD * 2;   // K or V: [128 kv x HD]
@@ -245,10 +276,15 @@ struct AttnBwdParams {
   long long dstride_b, dstride_s, dstride_h;
   int B, H, S, causal;
   float scale_log2, scale;
+  const int* doc_start;   // int32 [B, S], DOC kernels only
 };
 
-template <int HD>
-__global__ void __launch_bounds__(AttnCfg<HD>::THREADS, 1)
+// DOC: the query blocks of KV block j end at the first block whose first row starts its document after the block's last
+// key (binary search, doc_start is non-decreasing).  Inside the range P = 0 where key < doc_start[query]; since doc_start is
+// monotone, those queries are a suffix for each key row, so a thread keeps one bound per kv row instead of loading
+// doc_start per query column.
+template <int HD, bool DOC>
+__global__ void __launch_bounds__(BwdLayout<HD, DOC>::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
                 const AttnBwdParams p) {
@@ -284,16 +320,28 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   }
   __syncthreads();
   pdl_wait();
+  int i_end = nqb;   // producer and consumers walk the same query blocks [i0, i_end)
+  const int* ds_b = DOC ? p.doc_start + (size_t)b * p.S : nullptr;
+  if constexpr (DOC) {
+    const int last_key = j * BKV + BKV - 1;
+    int lo = i0;   // block i0 starts at key j * BKV and sees itself: the range is never empty
+    while (lo < i_end) {
+      const int mid = (lo + i_end) >> 1;
+      if (__ldg(ds_b + mid * BQB) > last_key) i_end = mid;
+      else lo = mid + 1;
+    }
+  }
 
-  if (HD == 64 ? warp == 8 : warp >= 8) {   // producer: warp 8 (D = 64) / warpgroup 2 (D = 128)
-    if constexpr (HD == 128) setmaxnreg_dec<24>();
-    if (lane == 0 && (HD == 64 || warp == 8)) {
+  constexpr bool WGP = BwdLayout<HD, DOC>::WG_PRODUCER;
+  if (WGP ? warp >= 8 : warp == 8) {   // producer: warpgroup 2 (setmaxnreg) / warp 8
+    if constexpr (WGP) setmaxnreg_dec<24>();
+    if (lane == 0 && warp == 8) {
       mbar_expect_tx(kv_full, 2 * L::KV_BYTES);
 #pragma unroll
       for (int c = 0; c < NC; ++c) tma_load_4d(smem + L::SB_K + c * CHUNK, &tmap_k, kv_full, c * 64, j * BKV, h, b);
 #pragma unroll
       for (int c = 0; c < NC; ++c) tma_load_4d(smem + L::SB_V + c * CHUNK, &tmap_v, kv_full, c * 64, j * BKV, h, b);
-      for (int i = i0, it = 0; i < nqb; ++i, ++it) {
+      for (int i = i0, it = 0; i < i_end; ++i, ++it) {
         const int st = it % Q_STAGES;
         mbar_wait(&q_empty[st], ((it / Q_STAGES) & 1) ^ 1);
         mbar_expect_tx(&q_full[st], 2 * L::QB_BYTES);
@@ -308,7 +356,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     pdl_trigger();
     return;
   }
-  if constexpr (HD == 128) setmaxnreg_inc<240>();
+  if constexpr (WGP) setmaxnreg_inc<240>();
 
   const int wg = warp >> 2;
   const int g = lane >> 2, q = lane & 3;
@@ -321,8 +369,22 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   float dv[HD / 2], dk[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+  int qend[2] = {0, 0};   // DOC: first query whose document starts after kv row r0 + 8 hr (from there on P = 0)
+  if constexpr (DOC) {
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int key = j * BKV + wg * 64 + r0 + 8 * hr;
+      int lo = key + 1, hi = i_end * BQB;   // doc_start[key] <= key; no query at or past i_end * BQB sees this block
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(ds_b + mid) > key) hi = mid;
+        else lo = mid + 1;
+      }
+      qend[hr] = lo;
+    }
+  }
   mbar_wait(kv_full, 0);
-  for (int i = i0, it = 0; i < nqb; ++i, ++it) {
+  for (int i = i0, it = 0; i < i_end; ++i, ++it) {
     const int st = it % Q_STAGES;
     mbar_wait(&q_full[st], (it / Q_STAGES) & 1);
     const uint32_t sq = smem_u32(smem + L::SB_Q + st * L::QB_BYTES), sdo = smem_u32(smem + L::SB_DO + st * L::QB_BYTES);
@@ -341,6 +403,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     fence_regs(s);
     fence_regs(dp);
     const bool masked = p.causal && i * BQB < j * BKV + BKV;   // query block overlaps the kv block
+    const bool dmask = DOC && i * BQB + BQB > min(qend[0], qend[1]);   // some query of the block is past a kv row's document
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
@@ -353,6 +416,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           const int idx = 4 * jj + 2 * hr + e1;
           float pv = exp2f(s[idx] * p.scale_log2 - L2);
           if (masked && i * BQB + qt < j * BKV + wg * 64 + r0 + 8 * hr) pv = 0.f;
+          if (dmask && i * BQB + qt >= qend[hr]) pv = 0.f;
           s[idx] = pv;
           dp[idx] = pv * (dp[idx] - dl);
         }
@@ -511,9 +575,20 @@ extern "C" int tepd_make_tmap_bshd(CUtensorMap* out, const void* ptr, int B, int
 
 namespace {
 
+template <auto Kern>
+cudaError_t set_smem(int bytes) {   // once per kernel instantiation
+  static bool cfg = false;
+  if (!cfg) {
+    cudaError_t e = cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e != cudaSuccess) return e;
+    cfg = true;
+  }
+  return cudaSuccess;
+}
+
 template <int HD>
 int attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, int B, int H, int S, float scale, int causal,
-             long long stride_b, long long stride_s, long long stride_h, cudaStream_t stream) {
+             long long stride_b, long long stride_s, long long stride_h, const int* doc_start, cudaStream_t stream) {
   CUtensorMap tq, tk, tv;
   int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, HD, stride_b, stride_s, stride_h, BQ);
   if (rc) return 100 + rc;
@@ -521,16 +596,15 @@ int attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, in
   if (rc) return 200 + rc;
   rc = tepd_make_tmap_bshd(&tv, v, B, S, H, HD, stride_b, stride_s, stride_h, BKV);
   if (rc) return 300 + rc;
-  static bool cfg = false;
-  if (!cfg) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem<HD>::BYTES);
-    if (e != cudaSuccess) return (int)e;
-    cfg = true;
-  }
+  auto kern = doc_start ? attn_fwd_kernel<HD, true> : attn_fwd_kernel<HD, false>;
+  cudaError_t e = doc_start ? set_smem<attn_fwd_kernel<HD, true>>(FwdSmem<HD>::BYTES)
+                            : set_smem<attn_fwd_kernel<HD, false>>(FwdSmem<HD>::BYTES);
+  if (e != cudaSuccess) return (int)e;
   AttnFwdParams p;
   p.O = o; p.lse = (float*)lse; p.B = B; p.H = H; p.S = S; p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
-  return (int)tepd::launch(attn_fwd_kernel<HD>, dim3((S / BQ) * B * H), dim3(AttnCfg<HD>::THREADS), FwdSmem<HD>::BYTES, stream,
+  p.doc_start = doc_start;
+  return (int)tepd::launch(kern, dim3((S / BQ) * B * H), dim3(AttnCfg<HD>::THREADS), FwdSmem<HD>::BYTES, stream,
                            tq, tk, tv, p);
 }
 
@@ -538,7 +612,7 @@ template <int HD>
 int attn_bwd(const void* dO, const void* q, const void* k, const void* v, const void* o, const void* lse, float* delta,
              float* dq_acc, void* dq, void* dk, void* dv, int B, int H, int S, float scale, int causal, long long stride_b,
              long long stride_s, long long stride_h, long long dstride_b, long long dstride_s, long long dstride_h,
-             cudaStream_t st) {
+             const int* doc_start, cudaStream_t st) {
   CUtensorMap tq, tk, tv, tdo;
   int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, HD, stride_b, stride_s, stride_h, BQB);
   if (rc) return 100 + rc;
@@ -554,17 +628,17 @@ int attn_bwd(const void* dO, const void* q, const void* k, const void* v, const 
                                   (const __nv_bfloat16*)dO, (const __nv_bfloat16*)o, delta, B, S, H);
     if (le != cudaSuccess) return (int)le;
   }
-  static bool cfg = false;
-  if (!cfg) {
-    cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem<HD>::BYTES);
-    if (e != cudaSuccess) return (int)e;
-    cfg = true;
-  }
+  auto kern = doc_start ? attn_bwd_kernel<HD, true> : attn_bwd_kernel<HD, false>;
+  cudaError_t e = doc_start ? set_smem<attn_bwd_kernel<HD, true>>(BwdSmem<HD>::BYTES)
+                            : set_smem<attn_bwd_kernel<HD, false>>(BwdSmem<HD>::BYTES);
+  if (e != cudaSuccess) return (int)e;
   AttnBwdParams p;
   p.lse = (const float*)lse; p.delta = delta; p.dq_acc = dq_acc; p.dk = dk; p.dv = dv;
   p.dstride_b = dstride_b; p.dstride_s = dstride_s; p.dstride_h = dstride_h;
   p.B = B; p.H = H; p.S = S; p.causal = causal; p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
-  cudaError_t le = tepd::launch(attn_bwd_kernel<HD>, dim3((S / BKV) * B * H), dim3(AttnCfg<HD>::THREADS), BwdSmem<HD>::BYTES, st,
+  p.doc_start = doc_start;
+  const int threads = doc_start ? BwdLayout<HD, true>::THREADS : BwdLayout<HD, false>::THREADS;
+  cudaError_t le = tepd::launch(kern, dim3((S / BKV) * B * H), dim3(threads), BwdSmem<HD>::BYTES, st,
                                 tq, tk, tv, tdo, p);
   if (le != cudaSuccess) return (int)le;
   return (int)tepd::launch(attn_dq_cast_kernel<HD>, dim3(tepd::num_sms() * 4), dim3(256), 0, st, dq_acc, (__nv_bfloat16*)dq, B, S,
@@ -574,13 +648,14 @@ int attn_bwd(const void* dO, const void* q, const void* k, const void* v, const 
 }  // namespace
 
 // q, k, v: bf16 pointers addressed as [B, S, H, D] with the given element strides (shared by q/k/v).  D = 64 or 128.
+// doc_start: nullptr, or int32 [B, S] non-decreasing document starts (causal only): query s sees keys [doc_start[b, s], s].
 extern "C" int tepd_attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, int B, int H, int S, int D,
                              float scale, int causal, long long stride_b, long long stride_s, long long stride_h,
-                             void* stream) {
-  if (S % 128 != 0) return -2;
+                             void* stream, const int* doc_start) {
+  if (S % 128 != 0 || (doc_start && !causal)) return -2;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (D == 64) return attn_fwd<64>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, st);
-  if (D == 128) return attn_fwd<128>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, st);
+  if (D == 64) return attn_fwd<64>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, doc_start, st);
+  if (D == 128) return attn_fwd<128>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, doc_start, st);
   return -2;
 }
 
@@ -588,8 +663,8 @@ extern "C" int tepd_attn_fwd(const void* q, const void* k, const void* v, void* 
 extern "C" int tepd_attn_bwd(const void* dO, const void* q, const void* k, const void* v, const void* o, const void* lse,
                              void* dq_acc, void* dq, void* dk, void* dv, int B, int H, int S, int D, float scale,
                              int causal, long long stride_b, long long stride_s, long long stride_h, long long dstride_b,
-                             long long dstride_s, long long dstride_h, void* stream) {
-  if ((D != 64 && D != 128) || S % 128 != 0) return -2;
+                             long long dstride_s, long long dstride_h, void* stream, const int* doc_start) {
+  if ((D != 64 && D != 128) || S % 128 != 0 || (doc_start && !causal)) return -2;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   static float* delta_buf = nullptr;
   static size_t delta_cap = 0;
@@ -614,7 +689,7 @@ extern "C" int tepd_attn_bwd(const void* dO, const void* q, const void* k, const
   }
   if (D == 64)
     return attn_bwd<64>(dO, q, k, v, o, lse, delta_buf, (float*)dq_acc, dq, dk, dv, B, H, S, scale, causal, stride_b, stride_s,
-                        stride_h, dstride_b, dstride_s, dstride_h, st);
+                        stride_h, dstride_b, dstride_s, dstride_h, doc_start, st);
   return attn_bwd<128>(dO, q, k, v, o, lse, delta_buf, (float*)dq_acc, dq, dk, dv, B, H, S, scale, causal, stride_b, stride_s,
-                       stride_h, dstride_b, dstride_s, dstride_h, st);
+                       stride_h, dstride_b, dstride_s, dstride_h, doc_start, st);
 }

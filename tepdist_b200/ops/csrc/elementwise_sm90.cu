@@ -385,13 +385,15 @@ __global__ void __launch_bounds__(256) colsum_kernel(const bf16* __restrict__ in
 }
 
 // ------------------------------------------------------------------ embedding
+// DOC (per-document positions): token t takes position t % S - ds[t], its offset inside its document.
+template <bool DOC>
 __global__ void embedding_fwd_kernel(const int* __restrict__ tok, const bf16* __restrict__ wte, const bf16* __restrict__ wpe,
-                                     bf16* __restrict__ out, int T, int S, int C) {
+                                     bf16* __restrict__ out, int T, int S, int C, const int* __restrict__ ds) {
   const int nvec = C >> 3;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)T * nvec;
        i += (size_t)gridDim.x * blockDim.x) {
     const int t = i / nvec, v = i % nvec;
-    const int id = tok[t], pos = t % S;
+    const int id = tok[t], pos = DOC ? t % S - ds[t] : t % S;
     float a[8], b[8];
     unpack8(__ldg(reinterpret_cast<const uint4*>(wte + (size_t)id * C) + v), a);
     unpack8(__ldg(reinterpret_cast<const uint4*>(wpe + (size_t)pos * C) + v), b);
@@ -400,13 +402,14 @@ __global__ void embedding_fwd_kernel(const int* __restrict__ tok, const bf16* __
     reinterpret_cast<uint4*>(out + (size_t)t * C)[v] = pack8(a);
   }
 }
+template <bool DOC>
 __global__ void embedding_bwd_kernel(const int* __restrict__ tok, const bf16* __restrict__ dout, float* __restrict__ dwte,
-                                     float* __restrict__ dwpe, int T, int S, int C) {
+                                     float* __restrict__ dwpe, int T, int S, int C, const int* __restrict__ ds) {
   const int nvec = C >> 3;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)T * nvec;
        i += (size_t)gridDim.x * blockDim.x) {
     const int t = i / nvec, v = i % nvec;
-    const int id = tok[t], pos = t % S;
+    const int id = tok[t], pos = DOC ? t % S - ds[t] : t % S;
     float d[8];
     unpack8(__ldg(reinterpret_cast<const uint4*>(dout + (size_t)t * C) + v), d);
     float* pe = dwte + (size_t)id * C + v * 8;
@@ -415,6 +418,36 @@ __global__ void embedding_bwd_kernel(const int* __restrict__ tok, const bf16* __
     asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(pe + 4), "f"(d[4]), "f"(d[5]), "f"(d[6]), "f"(d[7]) : "memory");
     asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(pp), "f"(d[0]), "f"(d[1]), "f"(d[2]), "f"(d[3]) : "memory");
     asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(pp + 4), "f"(d[4]), "f"(d[5]), "f"(d[6]), "f"(d[7]) : "memory");
+  }
+}
+
+// Document starts of packed rows: out[b, s] = 1 + the last p < s with tok[b, p] == eot, or 0.  One CTA per row walks it in
+// 256-token chunks: an inclusive max-scan of (tok[s - 1] == eot ? s : 0) plus the running maximum of the earlier chunks.
+__global__ void __launch_bounds__(256) doc_starts_kernel(const int* __restrict__ tok, int* __restrict__ out, int S, int eot) {
+  __shared__ int wmax[8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int* t = tok + (size_t)blockIdx.x * S;
+  int* o = out + (size_t)blockIdx.x * S;
+  int carry = 0;
+  for (int base = 0; base < S; base += 256) {
+    const int s = base + threadIdx.x;
+    int v = (s > 0 && s < S && t[s - 1] == eot) ? s : 0;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, v, off);
+      if (lane >= off) v = max(v, u);
+    }
+    if (lane == 31) wmax[warp] = v;
+    __syncthreads();
+    int before = carry, total = carry;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) {
+      if (w < warp) before = max(before, wmax[w]);
+      total = max(total, wmax[w]);
+    }
+    if (s < S) o[s] = max(before, v);
+    carry = total;
+    __syncthreads();   // wmax is rewritten by the next chunk
   }
 }
 
@@ -706,16 +739,29 @@ extern "C" int tepd_colsum(const void* in, void* out, int rows, int C, void* str
   return (int)tepd::launch(colsum_kernel, grid, dim3(256), 0, CS(stream), (const bf16*)in, (float*)out, rows, C, rpb);
   return (int)cudaGetLastError();
 }
+// doc_start: nullptr (position = t % S) or int32 [T] document starts (position = t % S - doc_start[t])
 extern "C" int tepd_embedding_fwd(const void* tok, const void* wte, const void* wpe, void* out, int T, int S, int C,
-                                  void* stream) {
+                                  void* stream, const int* doc_start) {
   if (C % 8) return -2;
-  embedding_fwd_kernel<<<grid_for((size_t)T * C / 8, 256), 256, 0, CS(stream)>>>((const int*)tok, (const bf16*)wte, (const bf16*)wpe, (bf16*)out, T, S, C);
+  if (doc_start)
+    embedding_fwd_kernel<true><<<grid_for((size_t)T * C / 8, 256), 256, 0, CS(stream)>>>((const int*)tok, (const bf16*)wte, (const bf16*)wpe, (bf16*)out, T, S, C, doc_start);
+  else
+    embedding_fwd_kernel<false><<<grid_for((size_t)T * C / 8, 256), 256, 0, CS(stream)>>>((const int*)tok, (const bf16*)wte, (const bf16*)wpe, (bf16*)out, T, S, C, nullptr);
   return (int)cudaGetLastError();
 }
 extern "C" int tepd_embedding_bwd(const void* tok, const void* dout, void* dwte, void* dwpe, int T, int S, int C,
-                                  void* stream) {
+                                  void* stream, const int* doc_start) {
   if (C % 8) return -2;
-  embedding_bwd_kernel<<<grid_for((size_t)T * C / 8, 256), 256, 0, CS(stream)>>>((const int*)tok, (const bf16*)dout, (float*)dwte, (float*)dwpe, T, S, C);
+  if (doc_start)
+    embedding_bwd_kernel<true><<<grid_for((size_t)T * C / 8, 256), 256, 0, CS(stream)>>>((const int*)tok, (const bf16*)dout, (float*)dwte, (float*)dwpe, T, S, C, doc_start);
+  else
+    embedding_bwd_kernel<false><<<grid_for((size_t)T * C / 8, 256), 256, 0, CS(stream)>>>((const int*)tok, (const bf16*)dout, (float*)dwte, (float*)dwpe, T, S, C, nullptr);
+  return (int)cudaGetLastError();
+}
+// tok, out: int32 [B, S]
+extern "C" int tepd_doc_starts(const void* tok, void* out, int B, int S, int eot, void* stream) {
+  if (B <= 0 || S <= 0) return -2;
+  doc_starts_kernel<<<B, 256, 0, CS(stream)>>>((const int*)tok, (int*)out, S, eot);
   return (int)cudaGetLastError();
 }
 extern "C" int tepd_xent_fwd_bwd(void* logits, const void* labels, void* loss_rows, void* loss_sum, int T, int V, int Vp,

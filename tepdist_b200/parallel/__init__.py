@@ -281,6 +281,16 @@ def build_pipeline(graph: Graph, trainer, stages: int, micro: int, comm_mode: st
     return PipelineRunner(worker, tasks, trainer.device)
 
 
+def check_context_parallel(graph: Graph, strategy: str) -> None:
+    """Context parallelism splits the sequence through attention with a K / V ring that knows nothing of document starts:
+    refuse "cp" and mesh strategies with a "cp" level for graphs with document-masked attention."""
+    mesh = _parse_mesh_strategy(strategy)
+    wants_cp = strategy == "cp" or (mesh is not None and "cp" in mesh[1])
+    if wants_cp and any(n.op == "attention" and len(n.inputs) > 1 for n in graph.nodes):
+        raise ValueError(f"strategy {strategy!r}: context parallelism does not support document-masked attention "
+                         "(eot_token / doc_starts); use dp, tp, pp or auto")
+
+
 def plan_and_build(graph: Graph, trainer, strategy: str, comm_mode: str, use_cuda_graph: bool, seed: int):
     from ..runtime.executor import Executor
     from .. import config

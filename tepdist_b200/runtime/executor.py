@@ -1287,12 +1287,14 @@ class Executor:
             return [t]
         if op == "constant":
             return [torch.full(n.outputs[0].shape, a["value"], dtype=torch_dtype(n.outputs[0].dtype, dev), device=dev)]
+        if op == "doc_starts":
+            return [ops.doc_starts(ins[0], a["eot"])]
         if op == "embedding":
-            return [ops.embedding_fwd(ins[0], ins[1], ins[2])]
+            return [ops.embedding_fwd(ins[0], ins[1], ins[2], doc_start=ins[3] if len(ins) > 3 else None)]
         if op == "embedding_bwd":
             dwte = self._grad_out(n, 0, n.outputs[0].shape)
             dwpe = self._grad_out(n, 1, n.outputs[1].shape)
-            ops.embedding_bwd(ins[0], ins[1], dwte, dwpe)
+            ops.embedding_bwd(ins[0], ins[1], dwte, dwpe, doc_start=ins[2] if len(ins) > 2 else None)
             return [dwte, dwpe]
         if op == "layernorm":
             y, mean, rstd = ops.layernorm_fwd(ins[0].contiguous(), ins[1], ins[2], a.get("eps", 1e-5))
@@ -1366,14 +1368,19 @@ class Executor:
             H = a["heads"]
             D = C3 // 3 // H
             q5 = qkv.view(B, S, H, 3, D)  # heads-major: a last-dim split is a split over heads
+            ds = ins[1] if len(ins) > 1 else None
             ring = self._ring(n)
             if ring is not None:    # context parallel: S is this rank's block of the sequence, K / V blocks ride the ring
+                if ds is not None:
+                    raise NotImplementedError("context parallelism (K / V ring) with document-masked attention")
                 o, lse = ring.forward(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], causal=a.get("causal", True))
                 return [o.reshape(B, S, H * D), lse]
-            o, lse = ops.attention_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], causal=a.get("causal", True))
+            o, lse = ops.attention_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], causal=a.get("causal", True),
+                                       doc_start=ds)
             return [o.view(B, S, H * D), lse]
         if op == "attention_bwd":
-            do, qkv, o, lse = ins
+            do, qkv, o, lse = ins[:4]
+            ds = ins[4] if len(ins) > 4 else None
             B, S, C3 = qkv.shape
             H = a["heads"]
             D = C3 // 3 // H
@@ -1381,11 +1388,13 @@ class Executor:
             dqkv = torch.empty(B, S, H, 3, D, dtype=qkv.dtype, device=dev)
             ring = self._ring(n)
             if ring is not None:
+                if ds is not None:
+                    raise NotImplementedError("context parallelism (K / V ring) with document-masked attention")
                 ring.backward(do.reshape(B, S, H, D), q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], o.reshape(B, S, H, D), lse,
                               causal=a.get("causal", True), dqkv_out=dqkv)
                 return [dqkv.view(B, S, C3)]
             ops.attention_bwd(do.reshape(B, S, H, D), q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], o.reshape(B, S, H, D),
-                              lse, causal=a.get("causal", True), dqkv_out=dqkv)
+                              lse, causal=a.get("causal", True), dqkv_out=dqkv, doc_start=ds)
             return [dqkv.view(B, S, C3)]
         if op == "softmax_xent":
             logits, labels = ins
