@@ -1,6 +1,8 @@
 // Persistent warp-specialised GEMM for sm_90a: TMA -> smem (SWIZZLE_128B, multi-stage mbarrier ring) -> wgmma.mma_async
 // into register accumulators of two consumer warpgroups -> epilogue from the accumulator fragments (bias / GELU /
-// residual / fp32 split-K or stream-K reduction fused).  bf16 operands, and e4m3 operands for the MoE expert GEMMs
+// residual / fp32 split-K or stream-K reduction fused).  bf16 outputs whose layout TMA can address go through a swizzled
+// shared-memory staging buffer and TMA stores that overlap the next tile's MMAs; the other outputs are stored straight
+// from the fragments.  bf16 operands, and e4m3 operands for the MoE expert GEMMs
 // (tepd_gemm_fp8).  This is the device-op layer that replaces the reference's cuBLAS GemmThunk
 // (reference: tensorflow/compiler/xla/service/gpu/gemm_thunk.cc, SURVEY §2.H K8).
 //
@@ -23,7 +25,9 @@ namespace {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row (128 e4m3 elements for the fp8 kernel)
-constexpr int NUM_THREADS = 288;  // warps 0..7: two consumer warpgroups, warp 8: TMA producer
+constexpr int NUM_THREADS = 384;  // warpgroups 0, 1: consumers (232 registers), warpgroup 2: TMA producer (40)
+constexpr int CONSUMER_REGS = 232, PRODUCER_REGS = 40;   // 2 x 128 x 232 + 128 x 40 = 384 x 168, the launch allocation
+constexpr int STORE_BOX = 64;     // TMA store box: 64 columns (128 B, one swizzle row) x 64 rows = 8 KB
 
 struct GemmParams {
   int M, N, K, batch;
@@ -92,6 +96,9 @@ __device__ __forceinline__ void next_work(const GemmParams& p, int& cursor, int 
   }
 }
 
+// kept out of line: a trap inlined into the kernel stops ptxas from giving the consumers the registers of setmaxnreg.inc
+__device__ __noinline__ void trap_stream_k_timeout() { __trap(); }
+
 __device__ __forceinline__ float gelu_tanh_grad(float x) {
   const float k0 = 0.7978845608028654f, k1 = 0.044715f;
   float t;
@@ -106,18 +113,46 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   return 0.5f * x * (1.0f + t);
 }
 
-template <int BLOCK_N>
+// Epilogue kinds, fixed at compile time.  EPI_DIRECT stores straight from the accumulator fragments and reads its options
+// (bias, GELU, GELU', residual, fp32 store, red.add, stream-K partials) at run time.  The other kinds write a bf16 output
+// through a shared-memory staging buffer (one 64 x BLOCK_N buffer per consumer warpgroup, in the TMA store box layout) and
+// TMA stores; their inputs are in shared memory before the epilogue starts: the bias (zeros when there is none) is copied
+// there at the start of the tile, the residual / GELU' aux tile is TMA-loaded into the staging buffer itself.
+enum Epi : int {
+  EPI_DIRECT = 0,
+  EPI_PLAIN,       // alpha * acc
+  EPI_BIAS,        // + bias
+  EPI_BIAS_RES,    // + bias + residual
+  EPI_GELU_DUAL,   // D = alpha * acc + bias, D2 = GELU(D)
+  EPI_GELU_BWD,    // alpha * acc * GELU'(aux)
+};
+template <int EPI> __host__ __device__ constexpr bool epi_bias() { return EPI == EPI_BIAS || EPI == EPI_BIAS_RES || EPI == EPI_GELU_DUAL; }
+template <int EPI> __host__ __device__ constexpr bool epi_tile_in() { return EPI == EPI_BIAS_RES || EPI == EPI_GELU_BWD; }
+
+// At BLOCK_N = 256 the 64 KB of staging cost one pipeline stage (3 x 48 KB + 64 KB + 2 KB of bias of the 227 KB).
+template <int BLOCK_N, bool STAGED>
 struct Cfg {
   static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
   static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BLOCK_N == 256) ? 4 : 6;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int STAGES = (BLOCK_N == 256) ? (STAGED ? 3 : 4) : 6;
+  static constexpr int STAGING_WG_BYTES = STAGED ? 64 * BLOCK_N * 2 : 0;
+  static constexpr int STAGING_OFF = STAGES * STAGE_BYTES;
+  static constexpr int BIAS_OFF = STAGING_OFF + 2 * STAGING_WG_BYTES;   // fp32 [2][BLOCK_N]
+  static constexpr int BAR_OFF = BIAS_OFF + (STAGED ? 2 * BLOCK_N * 4 : 0);
+  static constexpr int SMEM_BYTES = BAR_OFF + 1024 /*align*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory");
 };
 
 __device__ __forceinline__ void st_bf16x2(void* p, float a, float b) { *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(a, b); }
-__device__ __forceinline__ float2 ld_bf16x2(const void* p) {
-  return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
+__device__ __forceinline__ float2 ldg_bf16x2(const void* p) {
+  return __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(p)));
+}
+
+// named barrier of one consumer warpgroup (ids 2, 3; id 1 spans both consumer warpgroups)
+__device__ __forceinline__ void wg_bar_sync(int wg) {
+  if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
+  else         asm volatile("bar.sync 3, 128;" ::: "memory");
 }
 
 // Epilogue math + store for two adjacent columns (col, col + 1) of one output row.  v0 / v1 already hold the scaled
@@ -126,7 +161,7 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, const GemmPara
                                               bool add_res) {
   if (add_bias) {
     if (p.bias_bf16) {
-      const float2 f = ld_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.bias) + (long long)b * p.bias_stride + col);
+      const float2 f = ldg_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.bias) + (long long)b * p.bias_stride + col);
       v0 += f.x; v1 += f.y;
     } else {
       const float2 f = __ldg(reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.bias) + (long long)b * p.bias_stride + col));
@@ -138,12 +173,12 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, const GemmPara
     if (p.D2 != nullptr) st_bf16x2(reinterpret_cast<__nv_bfloat16*>(p.D) + off, v0, v1);  // pre-activation for backward
     v0 = gelu_tanh(v0); v1 = gelu_tanh(v1);
   } else if (p.act == 2) {
-    const float2 f = ld_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.aux) + off);
+    const float2 f = ldg_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.aux) + off);
     v0 *= gelu_tanh_grad(f.x); v1 *= gelu_tanh_grad(f.y);
   }
   if (add_res) {
-    const float2 f = ld_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.residual) + (long long)b * p.stride_res +
-                               (long long)row * p.ld_res + col);
+    const float2 f = ldg_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.residual) + (long long)b * p.stride_res +
+                                (long long)row * p.ld_res + col);
     v0 += f.x; v1 += f.y;
   }
   if (!p.out_fp32) {
@@ -157,36 +192,39 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, const GemmPara
   }
 }
 
-// One k-block (BLOCK_K = 128 bytes of K) of this warpgroup's 64 x BLOCK_N accumulator: four wgmma k-steps per 128-column
-// half.  bf16 steps are k16, e4m3 steps k32: 32 bytes of K either way, so the descriptors advance alike.
+// One k-block (BLOCK_K = 128 bytes of K) of this warpgroup's 64 x BLOCK_N accumulator: four wgmma k-steps, each one
+// m64n256k16 (BLOCK_N = 256) or m64n128 (BLOCK_N = 128).  bf16 steps are k16, e4m3 steps k32: 32 bytes of K either way,
+// so the descriptors advance alike.  The B descriptor covers all BLOCK_N rows: K-major B rows follow each other in the
+// swizzled tile (SBO), MN-major B is BLOCK_N / 64 chunks of 64 columns LBO apart.
 template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8>
-__device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 128][64], uint32_t sa, uint32_t sb, int wg, bool first) {
+__device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 2], uint32_t sa, uint32_t sb, int wg, bool first) {
+  static_assert(BLOCK_N == 128 || (BLOCK_N == 256 && !FP8), "tile width");
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    uint64_t da;
+    uint64_t da, db;
     if constexpr (!A_MN) da = make_smem_desc_sw128(sa + wg * 64 * 128 + k * 32, 0, 1024);
     else                 da = make_smem_desc_sw128(sa + wg * 64 * BLOCK_K * 2 + k * 16 * 128, 64 * BLOCK_K * 2, 1024);
-#pragma unroll
-    for (int h = 0; h < BLOCK_N / 128; ++h) {
-      uint64_t db;
-      if constexpr (!B_MN) db = make_smem_desc_sw128(sb + h * 128 * 128 + k * 32, 0, 1024);
-      else                 db = make_smem_desc_sw128(sb + h * 2 * 64 * BLOCK_K * 2 + k * 16 * 128, 64 * BLOCK_K * 2, 1024);
-      const uint32_t scale_d = (first && k == 0) ? 0u : 1u;
-      if constexpr (FP8) wgmma_m64n128k32_e4m3_ss(acc[h], da, db, scale_d);
-      else               wgmma_m64n128k16_bf16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], da, db, scale_d);
-    }
+    if constexpr (!B_MN) db = make_smem_desc_sw128(sb + k * 32, 0, 1024);
+    else                 db = make_smem_desc_sw128(sb + k * 16 * 128, 64 * BLOCK_K * 2, 1024);
+    const uint32_t scale_d = (first && k == 0) ? 0u : 1u;
+    if constexpr (FP8)                 wgmma_m64n128k32_e4m3_ss(acc, da, db, scale_d);
+    else if constexpr (BLOCK_N == 256) wgmma_m64n256k16_bf16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, scale_d);
+    else                               wgmma_m64n128k16_bf16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, scale_d);
   }
 }
 
-// Warp roles: warps 0-7 = two consumer warpgroups (wgmma into registers, rows [64 wg, +64) of the 128-row tile, then the
-// epilogue straight from the accumulator fragments); warp 8 = TMA producer.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8>
-__device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const GemmParams& p) {
-  using C = Cfg<BLOCK_N>;
+// Warp roles: warpgroups 0, 1 = consumers (wgmma into registers, rows [64 wg, +64) of the 128-row tile, then the
+// epilogue); warpgroup 2 = TMA producer (one elected thread), which hands most of its registers to the consumers.
+template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8, int EPI>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap& tmap_d,
+                                          const CUtensorMap& tmap_d2, const CUtensorMap& tmap_in, const GemmParams& p) {
+  constexpr bool STAGED = EPI != EPI_DIRECT;
+  using C = Cfg<BLOCK_N, STAGED>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + C::BAR_OFF);
   uint64_t* empty_bar = full_bar + C::STAGES;
+  uint64_t* in_bar = empty_bar + C::STAGES;   // [2]: residual / aux tile of consumer warpgroup 0 / 1 has landed
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -194,6 +232,13 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if constexpr (STAGED) {
+      tma_prefetch_desc(&tmap_d);
+      if constexpr (EPI == EPI_GELU_DUAL) tma_prefetch_desc(&tmap_d2);
+      if constexpr (epi_tile_in<EPI>()) tma_prefetch_desc(&tmap_in);
+    }
+    mbar_init(&in_bar[0], 1);
+    mbar_init(&in_bar[1], 1);
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 2);   // one arrival per consumer warpgroup
@@ -204,9 +249,10 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
   pdl_wait();      // everything above overlapped the previous kernel's tail; its outputs are visible from here on
   pdl_trigger();   // persistent grid: the next kernel may be scheduled as these CTAs retire
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 8 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       int cursor, cend;
@@ -242,12 +288,18 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
         }
       }
     }
-  } else {
+    return;
+  }
+  {
     // ===================== consumers: MMA + epilogue =====================
+    setmaxnreg_inc<CONSUMER_REGS>();
     const int wg = warp >> 2;                 // rows [64 wg, 64 wg + 64) of the tile
     const int t128 = threadIdx.x & 127;
     const int g = lane >> 2, q = lane & 3;
     const int row_base = wg * 64 + (warp & 3) * 16 + g;   // + 8 for the second half of each fragment
+    uint8_t* staging = smem + C::STAGING_OFF + wg * C::STAGING_WG_BYTES;
+    float* sbias = reinterpret_cast<float*>(smem + C::BIAS_OFF) + wg * BLOCK_N;
+    uint32_t in_phase = 0;
     int stage = 0;
     uint32_t phase = 0;
     int cursor, cend;
@@ -259,7 +311,31 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
       const int m_blk = w.m_blk, n_blk = w.n_blk;
       const int b = w.b;
       const bool has_k = w.kb0 < w.kb1;
-      float acc[BLOCK_N / 128][64];
+      if constexpr (STAGED) {
+        // the previous tile's epilogue is done with the bias copy and the staging buffer (every thread of the warpgroup
+        // passed its last barrier); once its TMA stores have read the buffer, the next input tile may land in it
+        if constexpr (epi_bias<EPI>()) {
+          for (int c = t128; c < BLOCK_N; c += 128) {
+            const int col = n_blk * BLOCK_N + c;
+            float v = 0.f;
+            if (p.bias != nullptr && col < p.N)
+              v = p.bias_bf16 ? __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col))
+                              : __ldg(reinterpret_cast<const float*>(p.bias) + col);   // (bias_stride is 0 here)
+            sbias[c] = v;
+          }
+        }
+        if (t128 == 0) {
+          bulk_wait_group_read<0>();
+          if constexpr (epi_tile_in<EPI>()) {
+            mbar_expect_tx(&in_bar[wg], C::STAGING_WG_BYTES);
+#pragma unroll
+            for (int c = 0; c < BLOCK_N / STORE_BOX; ++c)
+              tma_load_3d(staging + c * (64 * 128), &tmap_in, &in_bar[wg], n_blk * BLOCK_N + c * STORE_BOX,
+                          m_blk * BLOCK_M + wg * 64, b);
+          }
+        }
+      }
+      float acc[BLOCK_N / 2];
       int prev = -1;
       for (int kb = w.kb0; kb < w.kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
@@ -273,12 +349,69 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
         if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
-#pragma unroll
-      for (int h = 0; h < BLOCK_N / 128; ++h) fence_regs(acc[h]);
+      fence_regs(acc);
       if (prev >= 0 && t128 == 0) mbar_arrive(&empty_bar[prev]);
 
       const bool add_bias = p.bias != nullptr && w.lead;
       const bool add_res = p.residual != nullptr && w.lead;
+      if constexpr (STAGED) {
+        // bf16 tile -> swizzled staging buffer (the TMA store box layout: 64-column boxes of 64 rows x 128 B, 16-byte
+        // chunk c of row r at chunk c ^ (r & 7)) -> TMA stores.  A thread reads its residual / aux pair from the address it
+        // then overwrites.  The stores drain while this warpgroup runs the next tile's MMAs.  Rows / columns outside the
+        // output are not written here and clipped by the store.  The dual-output GELU epilogue stores D, then D2.
+        if constexpr (epi_tile_in<EPI>()) {
+          mbar_wait(&in_bar[wg], in_phase);
+          in_phase ^= 1;
+        }
+        wg_bar_sync(wg);   // the bias copy is visible
+        if (has_k) {
+#pragma unroll
+          for (int r = 0; r < (EPI == EPI_GELU_DUAL ? 2 : 1); ++r) {
+            if (r == 1) {
+              if (t128 == 0) bulk_wait_group_read<0>();
+              wg_bar_sync(wg);
+            }
+#pragma unroll
+            for (int hr = 0; hr < 2; ++hr) {
+              const int row_in_tile = row_base + hr * 8;
+              if (m_blk * BLOCK_M + row_in_tile >= p.M) continue;
+              const uint32_t srow = smem_u32(staging) + (row_in_tile - wg * 64) * 128;
+#pragma unroll
+              for (int j = 0; j < BLOCK_N / 8; ++j) {
+                const int cit = j * 8 + 2 * q;
+                if (n_blk * BLOCK_N + cit >= p.N) continue;
+                const uint32_t addr = srow + (j / 8) * (64 * 128) + (((j & 7) ^ g) << 4) + 4 * q;
+                float v0 = acc[4 * j + 2 * hr] * p.alpha, v1 = acc[4 * j + 2 * hr + 1] * p.alpha;
+                if constexpr (epi_bias<EPI>()) {
+                  const float2 bb = *reinterpret_cast<const float2*>(sbias + cit);
+                  v0 += bb.x; v1 += bb.y;
+                }
+                if constexpr (EPI == EPI_GELU_DUAL) {
+                  if (r == 1) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
+                }
+                if constexpr (epi_tile_in<EPI>()) {
+                  uint32_t in;
+                  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(in) : "r"(addr));
+                  const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&in));
+                  if constexpr (EPI == EPI_GELU_BWD) { v0 *= gelu_tanh_grad(f.x); v1 *= gelu_tanh_grad(f.y); }
+                  else                               { v0 += f.x; v1 += f.y; }
+                }
+                asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)));
+              }
+            }
+            fence_proxy_async();   // the generic-proxy writes above are read by the TMA unit
+            wg_bar_sync(wg);
+            if (t128 == 0) {
+#pragma unroll
+              for (int c = 0; c < BLOCK_N / STORE_BOX; ++c)
+                tma_store_3d(r == 1 ? &tmap_d2 : &tmap_d, staging + c * (64 * 128), n_blk * BLOCK_N + c * STORE_BOX,
+                             m_blk * BLOCK_M + wg * 64, b);
+              bulk_commit_group();
+            }
+          }
+        }
+        continue;
+      }
       // stream-K units that cover only part of a tile's K range (outputs with a real epilogue): a unit that starts
       // mid-tile (always a CTA's FIRST unit) stores its fp32 partial tile into workspace slot [blockIdx.x] and raises
       // flag[blockIdx.x]; the unit that holds k-block 0 (always a CTA's LAST unit) is the finisher: it waits for the
@@ -298,7 +431,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
             const long long t0 = clock64();
             do {
               asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(f) : "l"(p.sk_cnt + j) : "memory");
-              if (f == 0u && clock64() - t0 > 4000000000LL) __trap();   // a partner never arrived: fail loudly
+              if (f == 0u && clock64() - t0 > 4000000000LL) trap_stream_k_timeout();   // a partner never arrived: fail loudly
             } while (f == 0u);
           }
         }
@@ -314,28 +447,25 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
           float alpha = p.alpha;
           if (scale_rows) alpha *= scale_rows[row] * p.w_scale[b];
 #pragma unroll
-          for (int h = 0; h < BLOCK_N / 128; ++h) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int cit = h * 128 + j * 8 + 2 * q;   // column inside the tile
-              const int col = n_blk * BLOCK_N + cit;
-              if (col >= p.N) continue;
-              float v0 = acc[h][4 * j + 2 * hr] * alpha, v1 = acc[h][4 * j + 2 * hr + 1] * alpha;
-              float* wp = p.sk_ws + ((long long)blockIdx.x * BLOCK_M + row_in_tile) * 256 + cit;
-              if (sk_store) {
-                *reinterpret_cast<float2*>(wp) = make_float2(v0, v1);
-                continue;
-              }
-              if (sk_finish) {
-                for (int jj = blockIdx.x + 1; jj < partner_end; ++jj) {
-                  float2 t;
-                  asm volatile("ld.global.cg.v2.f32 {%0,%1}, [%2];" : "=f"(t.x), "=f"(t.y)
-                               : "l"(p.sk_ws + ((long long)jj * BLOCK_M + row_in_tile) * 256 + cit));
-                  v0 += t.x; v1 += t.y;
-                }
-              }
-              epilogue_pair(v0, v1, p, row, col, b, add_bias, add_res);
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const int cit = j * 8 + 2 * q;   // column inside the tile
+            const int col = n_blk * BLOCK_N + cit;
+            if (col >= p.N) continue;
+            float v0 = acc[4 * j + 2 * hr] * alpha, v1 = acc[4 * j + 2 * hr + 1] * alpha;
+            float* wp = p.sk_ws + ((long long)blockIdx.x * BLOCK_M + row_in_tile) * 256 + cit;
+            if (sk_store) {
+              *reinterpret_cast<float2*>(wp) = make_float2(v0, v1);
+              continue;
             }
+            if (sk_finish) {
+              for (int jj = blockIdx.x + 1; jj < partner_end; ++jj) {
+                float2 t;
+                asm volatile("ld.global.cg.v2.f32 {%0,%1}, [%2];" : "=f"(t.x), "=f"(t.y)
+                             : "l"(p.sk_ws + ((long long)jj * BLOCK_M + row_in_tile) * 256 + cit));
+                v0 += t.x; v1 += t.y;
+              }
+            }
+            epilogue_pair(v0, v1, p, row, col, b, add_bias, add_res);
           }
         }
       }
@@ -351,14 +481,18 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
         }
       }
     }
+    if constexpr (STAGED) {
+      if (t128 == 0) bulk_wait_group<0>();   // the staging buffers live until the last stores have read them
+    }
   }
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8>
+template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const GemmParams p) {
-  gemm_body<BLOCK_N, A_MN, B_MN, FP8>(tmap_a, tmap_b, p);
+                 const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_d2,
+                 const __grid_constant__ CUtensorMap tmap_in, const GemmParams p) {
+  gemm_body<BLOCK_N, A_MN, B_MN, FP8, EPI>(tmap_a, tmap_b, tmap_d, tmap_d2, tmap_in, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -399,11 +533,12 @@ extern "C" int tepd_make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, long lo
   return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8 = false>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int num_sms,
-                       cudaStream_t stream) {
-  using C = Cfg<BLOCK_N>;
-  auto kern = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, FP8>;
+struct Maps { CUtensorMap a, b, d, d2, in; };
+
+template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8, int EPI>
+static int launch_gemm(const Maps& m, const GemmParams& p, int num_sms, cudaStream_t stream) {
+  using C = Cfg<BLOCK_N, EPI != EPI_DIRECT>;
+  auto kern = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, FP8, EPI>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
@@ -416,7 +551,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmP
     const long long iters = (long long)p.m_blocks * p.n_blocks * p.batch * p.k_blocks;
     grid = (int)((iters + p.stream_k - 1) / p.stream_k);
   }
-  return (int)tepd::launch(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, ta, tb, p);
+  return (int)tepd::launch(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, m.a, m.b, m.d, m.d2, m.in, p);
 }
 
 // C ABI entry (called from Python via ctypes).  All leading dims / strides are in elements.
@@ -505,14 +640,49 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
   if (!b_mn) rc = tepd_make_tmap_bf16_3d(&tb, B, K, N, batch, ldb, stride_b, BLOCK_K, block_n);
   else       rc = tepd_make_tmap_bf16_3d(&tb, B, N, K, batch, ldb, stride_b, 64, BLOCK_K);
   if (rc) return 200 + rc;
+  // Epilogue kind.  bf16 outputs go through shared memory and TMA when TMA can address the output and the residual / aux
+  // (16-byte aligned base, row pitch and batch stride; aux and D2 share D's layout) and a staged kind exists for the
+  // flags and the operand layout: plain for every layout, bias / bias + residual / dual GELU for the forward layout
+  // (A and B K-major), GELU' for the data-gradient layout (B MN-major).  Everything else stores from the fragments.
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  const bool fwd = !a_mn && !b_mn, dgrad = !a_mn && b_mn;
+  int epi = EPI_DIRECT;
+  if (!out_fp32 && p.stream_k == 0 && ldd % 8 == 0 && (batch == 1 || stride_d % 8 == 0) && al16(D)) {
+    const bool res_ok = residual != nullptr && al16(residual) && ld_res % 8 == 0 && (batch == 1 || stride_res % 8 == 0);
+    if (act == 0 && !bias && !residual) epi = EPI_PLAIN;
+    else if (act == 0 && !residual && fwd) epi = EPI_BIAS;
+    else if (act == 0 && res_ok && fwd) epi = EPI_BIAS_RES;
+    else if (act == 1 && D2 && al16(D2) && !residual && fwd) epi = EPI_GELU_DUAL;
+    else if (act == 2 && al16(aux) && !bias && !residual && dgrad) epi = EPI_GELU_BWD;
+  }
+  Maps m;
+  m.a = ta; m.b = tb;
+  m.d = m.d2 = m.in = CUtensorMap{};
+  if (epi != EPI_DIRECT) {
+    rc = tepd_make_tmap_bf16_3d(&m.d, D, N, M, batch, ldd, stride_d, STORE_BOX, 64);
+    if (!rc && epi == EPI_GELU_DUAL) rc = tepd_make_tmap_bf16_3d(&m.d2, D2, N, M, batch, ldd, stride_d, STORE_BOX, 64);
+    if (!rc && epi == EPI_BIAS_RES) rc = tepd_make_tmap_bf16_3d(&m.in, residual, N, M, batch, ld_res, stride_res, STORE_BOX, 64);
+    if (!rc && epi == EPI_GELU_BWD) rc = tepd_make_tmap_bf16_3d(&m.in, aux, N, M, batch, ldd, stride_d, STORE_BOX, 64);
+    if (rc) return 300 + rc;
+  }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-#define DISPATCH(BN)                                                                   \
-  if (!a_mn && !b_mn) return launch_gemm<BN, false, false>(ta, tb, p, num_sms, s);     \
-  if (!a_mn && b_mn) return launch_gemm<BN, false, true>(ta, tb, p, num_sms, s);       \
-  if (a_mn && !b_mn) return launch_gemm<BN, true, false>(ta, tb, p, num_sms, s);       \
-  return launch_gemm<BN, true, true>(ta, tb, p, num_sms, s);
-  if (block_n == 256) { DISPATCH(256) } else { DISPATCH(128) }
-#undef DISPATCH
+#define LAYOUTS(BN, E)                                                                \
+  if (!a_mn && !b_mn) return launch_gemm<BN, false, false, false, E>(m, p, num_sms, s); \
+  if (!a_mn && b_mn) return launch_gemm<BN, false, true, false, E>(m, p, num_sms, s);   \
+  if (a_mn && !b_mn) return launch_gemm<BN, true, false, false, E>(m, p, num_sms, s);   \
+  return launch_gemm<BN, true, true, false, E>(m, p, num_sms, s);
+#define KINDS(BN)                                                                                         \
+  switch (epi) {                                                                                          \
+    case EPI_PLAIN: { LAYOUTS(BN, EPI_PLAIN) }                                                            \
+    case EPI_BIAS: return launch_gemm<BN, false, false, false, EPI_BIAS>(m, p, num_sms, s);               \
+    case EPI_BIAS_RES: return launch_gemm<BN, false, false, false, EPI_BIAS_RES>(m, p, num_sms, s);       \
+    case EPI_GELU_DUAL: return launch_gemm<BN, false, false, false, EPI_GELU_DUAL>(m, p, num_sms, s);     \
+    case EPI_GELU_BWD: return launch_gemm<BN, false, true, false, EPI_GELU_BWD>(m, p, num_sms, s);        \
+    default: { LAYOUTS(BN, EPI_DIRECT) }                                                                  \
+  }
+  if (block_n == 256) { KINDS(256) } else { KINDS(128) }
+#undef KINDS
+#undef LAYOUTS
 }
 
 // ------------------------------------------------------------------ fp8 (e4m3) grouped GEMM for the MoE experts
@@ -539,8 +709,9 @@ extern "C" int tepd_gemm_fp8(const void* A, const void* B, void* D, const void* 
   p.D = D; p.bias = bias; p.residual = nullptr; p.alpha = 1.0f;
   p.out_fp32 = 0; p.accumulate = 0; p.act = act == 1 ? 1 : 0; p.bias_bf16 = 0; p.D2 = nullptr; p.aux = nullptr;
   p.row_scale = (const float*)row_scale; p.w_scale = (const float*)w_scale; p.bias_stride = N;
-  CUtensorMap ta, tb;
-  if (make_tmap_u8(&ta, A, K, M, batch, BLOCK_M) || make_tmap_u8(&tb, B, K, N, batch, BN)) return -3;
+  Maps m;
+  m.d = m.d2 = m.in = CUtensorMap{};
+  if (make_tmap_u8(&m.a, A, K, M, batch, BLOCK_M) || make_tmap_u8(&m.b, B, K, N, batch, BN)) return -3;
   if (num_sms <= 0) num_sms = tepd::num_sms();
-  return launch_gemm<BN, false, false, true>(ta, tb, p, num_sms, reinterpret_cast<cudaStream_t>(stream));
+  return launch_gemm<BN, false, false, true, EPI_DIRECT>(m, p, num_sms, reinterpret_cast<cudaStream_t>(stream));
 }
