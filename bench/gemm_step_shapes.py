@@ -9,10 +9,14 @@ calls per graph), so the host-side launch cost is not in the time; the zero-fill
 (the step zero-fills all such slots at once).  Times are CUDA-event means over enough replays to span `--window` ms
 after warm-up.  The card name, power limit and max SM clock are read in the same run.
 
-    python bench/gemm_step_shapes.py [--window 200] [--json out.json] [--compare DIR]
+    python bench/gemm_step_shapes.py [--window 200] [--json out.json] [--compare DIR] [--wgrad-breakdown]
 
 --compare DIR: the first run writes every GEMM output to DIR; a later run (another build) compares its outputs with those
 element by element and prints how many elements differ and by how much.
+
+--wgrad-breakdown: instead of the step table, time each weight-gradient shape four ways, plain stores without split-K,
+to tell the cost of the fp32 output from the cost of the MN-major A operand: A MN-major as the step runs it (dy [T, n_out])
+or K-major (dy^T made contiguous before timing), each with an fp32 output and with a bf16 output.
 """
 from __future__ import annotations
 
@@ -122,11 +126,47 @@ def cases(T: int = 4096, C: int = 1024, Vp: int = 50304, L: int = 24):
     return rows
 
 
+def wgrad_breakdown(window_ms: float, T: int = 4096, C: int = 1024, Vp: int = 50304) -> list:
+    """Weight-gradient shapes dW [n_out, k_in] = dy^T @ x, plain stores, four variants: (a) A MN-major, fp32 out (the
+    step's call when it stores); (b) A MN-major, bf16 out; (c) A K-major, fp32 out; (d) A K-major, bf16 out (the
+    data-gradient layout)."""
+    from tepdist_b200 import ops
+    print(f"{'wgrad':12s} {'M':>5} {'N':>5} {'K':>5} | {'(a) MN f32':>10} {'(b) MN bf16':>11} {'(c) K f32':>10} "
+          f"{'(d) K bf16':>10}  (ms per call)")
+    rows = []
+    for i, (name, n_out, k_in) in enumerate((("qkv", 3 * C, C), ("attn/c_proj", C, C), ("mlp/c_fc", 4 * C, C),
+                                             ("mlp/c_proj", C, 4 * C), ("lm_head", Vp, C))):
+        gen = torch.Generator(device="cuda")
+        gen.manual_seed(4321 + i)
+        dy = torch.randn(T, n_out, generator=gen, device="cuda").to(torch.bfloat16)
+        x = torch.randn(T, k_in, generator=gen, device="cuda").to(torch.bfloat16)
+        dyt = dy.t().contiguous()
+        r = {"wgrad": name, "M": n_out, "N": k_in, "K": T}
+        for key, a, a_mn, dt in (("a_mn_f32", dy, True, torch.float32), ("a_mn_bf16", dy, True, torch.bfloat16),
+                                 ("a_k_f32", dyt, False, torch.float32), ("a_k_bf16", dyt, False, torch.bfloat16)):
+            out = torch.empty(n_out, k_in, dtype=dt, device="cuda")
+
+            def ours(a=a, a_mn=a_mn, out=out):
+                ops.gemm(a, x, a_mn=a_mn, b_mn=True, out=out, split_k=1)
+            n0 = ops.launch_count()
+            ours()
+            assert ops.launch_count() > n0, f"{name}: our GEMM kernel did not run"
+            r[key] = _time_ms(ours, window_ms)
+            del out
+        print(f"{name:12s} {n_out:5d} {k_in:5d} {T:5d} | {r['a_mn_f32']:10.3f} {r['a_mn_bf16']:11.3f} {r['a_k_f32']:10.3f} "
+              f"{r['a_k_bf16']:10.3f}", flush=True)
+        rows.append(r)
+        del dy, x, dyt
+        torch.cuda.empty_cache()
+    return rows
+
+
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--window", type=float, default=200.0, help="ms of back-to-back calls per measurement")
     ap.add_argument("--json", default=None)
     ap.add_argument("--compare", metavar="DIR", default=None)
+    ap.add_argument("--wgrad-breakdown", action="store_true", help="time the weight-gradient shapes four ways (see above)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("gemm_step_shapes.py: no CUDA GPU; the timings are only meaningful on the H100")
@@ -134,6 +174,12 @@ def main() -> None:
     ops.lib()
     card = _card()
     print(f"# card: {card}  (name, power limit, max SM clock)")
+    if a.wgrad_breakdown:
+        rows = wgrad_breakdown(a.window)
+        if a.json:
+            with open(a.json, "w") as fh:
+                json.dump({"card": card, "wgrad_breakdown": rows}, fh, indent=1)
+        return
     print(f"{'gemm':18s} {'M':>5} {'N':>6} {'K':>6} {'epilogue':15s} {'calls':>5} | {'ours ms':>8} {'TFLOP/s':>7} | "
           f"{'cuBLAS ms':>9} {'TFLOP/s':>7} | {'calls x ours':>12} {'calls x cuBLAS':>14}")
     rows, tot, tot_ref = [], 0.0, 0.0

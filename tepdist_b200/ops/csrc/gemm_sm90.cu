@@ -1,8 +1,9 @@
 // Persistent warp-specialised GEMM for sm_90a: TMA -> smem (SWIZZLE_128B, multi-stage mbarrier ring) -> wgmma.mma_async
 // into register accumulators of two consumer warpgroups -> epilogue from the accumulator fragments (bias / GELU /
-// residual / fp32 split-K or stream-K reduction fused).  bf16 outputs whose layout TMA can address go through a swizzled
-// shared-memory staging buffer and TMA stores that overlap the next tile's MMAs; the other outputs are stored straight
-// from the fragments.  bf16 operands, and e4m3 operands for the MoE expert GEMMs
+// residual / fp32 split-K or stream-K reduction fused).  bf16 outputs, and the fp32 weight-gradient outputs, whose layout
+// TMA can address go through a swizzled shared-memory staging buffer and TMA stores (or TMA reduce-adds) that overlap the
+// next tile's MMAs; the other outputs are stored straight from the fragments.  bf16 operands, and e4m3 operands for the
+// MoE expert GEMMs
 // (tepd_gemm_fp8).  This is the device-op layer that replaces the reference's cuBLAS GemmThunk
 // (reference: tensorflow/compiler/xla/service/gpu/gemm_thunk.cc, SURVEY §2.H K8).
 //
@@ -28,6 +29,7 @@ constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row (128 e4m3 ele
 constexpr int NUM_THREADS = 384;  // warpgroups 0, 1: consumers (232 registers), warpgroup 2: TMA producer (40)
 constexpr int CONSUMER_REGS = 232, PRODUCER_REGS = 40;   // 2 x 128 x 232 + 128 x 40 = 384 x 168, the launch allocation
 constexpr int STORE_BOX = 64;     // TMA store box: 64 columns (128 B, one swizzle row) x 64 rows = 8 KB
+constexpr int STORE_BOX_F32 = 32; // the same 8 KB box for fp32 outputs: 32 columns (128 B) x 64 rows
 
 struct GemmParams {
   int M, N, K, batch;
@@ -114,10 +116,11 @@ __device__ __forceinline__ float gelu_tanh(float x) {
 }
 
 // Epilogue kinds, fixed at compile time.  EPI_DIRECT stores straight from the accumulator fragments and reads its options
-// (bias, GELU, GELU', residual, fp32 store, red.add, stream-K partials) at run time.  The other kinds write a bf16 output
-// through a shared-memory staging buffer (one 64 x BLOCK_N buffer per consumer warpgroup, in the TMA store box layout) and
-// TMA stores; their inputs are in shared memory before the epilogue starts: the bias (zeros when there is none) is copied
-// there at the start of the tile, the residual / GELU' aux tile is TMA-loaded into the staging buffer itself.
+// (bias, GELU, GELU', residual, fp32 store, red.add, stream-K partials) at run time.  The other kinds write their output
+// through a shared-memory staging buffer (one 64 x BLOCK_N bf16 buffer per consumer warpgroup, in the TMA store box layout)
+// and TMA stores; their inputs are in shared memory before the epilogue starts: the bias (zeros when there is none) is
+// copied there at the start of the tile, the residual / GELU' aux tile is TMA-loaded into the staging buffer itself.  The
+// fp32 kinds fill the same buffer with half the tile's columns at a time (64 x BLOCK_N / 2 fp32) and store it in two rounds.
 enum Epi : int {
   EPI_DIRECT = 0,
   EPI_PLAIN,       // alpha * acc
@@ -125,9 +128,12 @@ enum Epi : int {
   EPI_BIAS_RES,    // + bias + residual
   EPI_GELU_DUAL,   // D = alpha * acc + bias, D2 = GELU(D)
   EPI_GELU_BWD,    // alpha * acc * GELU'(aux)
+  EPI_F32,         // fp32 D = alpha * acc
+  EPI_F32_ADD,     // fp32 D += alpha * acc (TMA reduce-add: split-K, stream-K and gradient accumulation)
 };
 template <int EPI> __host__ __device__ constexpr bool epi_bias() { return EPI == EPI_BIAS || EPI == EPI_BIAS_RES || EPI == EPI_GELU_DUAL; }
 template <int EPI> __host__ __device__ constexpr bool epi_tile_in() { return EPI == EPI_BIAS_RES || EPI == EPI_GELU_BWD; }
+template <int EPI> __host__ __device__ constexpr bool epi_f32() { return EPI == EPI_F32 || EPI == EPI_F32_ADD; }
 
 // At BLOCK_N = 256 the 64 KB of staging cost one pipeline stage (3 x 48 KB + 64 KB + 2 KB of bias of the 227 KB).
 template <int BLOCK_N, bool STAGED>
@@ -358,7 +364,9 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
         // bf16 tile -> swizzled staging buffer (the TMA store box layout: 64-column boxes of 64 rows x 128 B, 16-byte
         // chunk c of row r at chunk c ^ (r & 7)) -> TMA stores.  A thread reads its residual / aux pair from the address it
         // then overwrites.  The stores drain while this warpgroup runs the next tile's MMAs.  Rows / columns outside the
-        // output are not written here and clipped by the store.  The dual-output GELU epilogue stores D, then D2.
+        // output are not written here and clipped by the store.  The dual-output GELU epilogue stores D, then D2.  The
+        // fp32 kinds store columns [0, BLOCK_N / 2) of the tile, then [BLOCK_N / 2, BLOCK_N), in 32-column boxes; the
+        // accumulate kind adds each box into the output with a TMA reduce-add (a stream-K or split-K unit adds its partial).
         if constexpr (epi_tile_in<EPI>()) {
           mbar_wait(&in_bar[wg], in_phase);
           in_phase ^= 1;
@@ -366,7 +374,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
         wg_bar_sync(wg);   // the bias copy is visible
         if (has_k) {
 #pragma unroll
-          for (int r = 0; r < (EPI == EPI_GELU_DUAL ? 2 : 1); ++r) {
+          for (int r = 0; r < (EPI == EPI_GELU_DUAL || epi_f32<EPI>() ? 2 : 1); ++r) {
             if (r == 1) {
               if (t128 == 0) bulk_wait_group_read<0>();
               wg_bar_sync(wg);
@@ -376,36 +384,56 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
               const int row_in_tile = row_base + hr * 8;
               if (m_blk * BLOCK_M + row_in_tile >= p.M) continue;
               const uint32_t srow = smem_u32(staging) + (row_in_tile - wg * 64) * 128;
+              if constexpr (epi_f32<EPI>()) {
+                // fragment column pair jj of this round: box jj / 4, 16-byte chunk 2 (jj & 3) + q / 2, 8 bytes in
 #pragma unroll
-              for (int j = 0; j < BLOCK_N / 8; ++j) {
-                const int cit = j * 8 + 2 * q;
-                if (n_blk * BLOCK_N + cit >= p.N) continue;
-                const uint32_t addr = srow + (j / 8) * (64 * 128) + (((j & 7) ^ g) << 4) + 4 * q;
-                float v0 = acc[4 * j + 2 * hr] * p.alpha, v1 = acc[4 * j + 2 * hr + 1] * p.alpha;
-                if constexpr (epi_bias<EPI>()) {
-                  const float2 bb = *reinterpret_cast<const float2*>(sbias + cit);
-                  v0 += bb.x; v1 += bb.y;
+                for (int jj = 0; jj < BLOCK_N / 16; ++jj) {
+                  const int j = r * (BLOCK_N / 16) + jj;
+                  if (n_blk * BLOCK_N + j * 8 + 2 * q >= p.N) continue;
+                  const uint32_t addr = srow + (jj / 4) * (64 * 128) + ((((jj & 3) * 2 + (q >> 1)) ^ g) << 4) + 8 * (q & 1);
+                  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(acc[4 * j + 2 * hr] * p.alpha),
+                               "f"(acc[4 * j + 2 * hr + 1] * p.alpha));
                 }
-                if constexpr (EPI == EPI_GELU_DUAL) {
-                  if (r == 1) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
+              } else {
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                  const int cit = j * 8 + 2 * q;
+                  if (n_blk * BLOCK_N + cit >= p.N) continue;
+                  const uint32_t addr = srow + (j / 8) * (64 * 128) + (((j & 7) ^ g) << 4) + 4 * q;
+                  float v0 = acc[4 * j + 2 * hr] * p.alpha, v1 = acc[4 * j + 2 * hr + 1] * p.alpha;
+                  if constexpr (epi_bias<EPI>()) {
+                    const float2 bb = *reinterpret_cast<const float2*>(sbias + cit);
+                    v0 += bb.x; v1 += bb.y;
+                  }
+                  if constexpr (EPI == EPI_GELU_DUAL) {
+                    if (r == 1) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
+                  }
+                  if constexpr (epi_tile_in<EPI>()) {
+                    uint32_t in;
+                    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(in) : "r"(addr));
+                    const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&in));
+                    if constexpr (EPI == EPI_GELU_BWD) { v0 *= gelu_tanh_grad(f.x); v1 *= gelu_tanh_grad(f.y); }
+                    else                               { v0 += f.x; v1 += f.y; }
+                  }
+                  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)));
                 }
-                if constexpr (epi_tile_in<EPI>()) {
-                  uint32_t in;
-                  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(in) : "r"(addr));
-                  const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&in));
-                  if constexpr (EPI == EPI_GELU_BWD) { v0 *= gelu_tanh_grad(f.x); v1 *= gelu_tanh_grad(f.y); }
-                  else                               { v0 += f.x; v1 += f.y; }
-                }
-                asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(pack_bf16x2(v0, v1)));
               }
             }
             fence_proxy_async();   // the generic-proxy writes above are read by the TMA unit
             wg_bar_sync(wg);
             if (t128 == 0) {
 #pragma unroll
-              for (int c = 0; c < BLOCK_N / STORE_BOX; ++c)
-                tma_store_3d(r == 1 ? &tmap_d2 : &tmap_d, staging + c * (64 * 128), n_blk * BLOCK_N + c * STORE_BOX,
-                             m_blk * BLOCK_M + wg * 64, b);
+              for (int c = 0; c < BLOCK_N / STORE_BOX; ++c) {
+                if constexpr (EPI == EPI_F32)
+                  tma_store_3d(&tmap_d, staging + c * (64 * 128), n_blk * BLOCK_N + r * (BLOCK_N / 2) + c * STORE_BOX_F32,
+                               m_blk * BLOCK_M + wg * 64, b);
+                else if constexpr (EPI == EPI_F32_ADD)
+                  tma_reduce_add_3d(&tmap_d, staging + c * (64 * 128), n_blk * BLOCK_N + r * (BLOCK_N / 2) + c * STORE_BOX_F32,
+                                    m_blk * BLOCK_M + wg * 64, b);
+                else
+                  tma_store_3d(r == 1 ? &tmap_d2 : &tmap_d, staging + c * (64 * 128), n_blk * BLOCK_N + c * STORE_BOX,
+                               m_blk * BLOCK_M + wg * 64, b);
+              }
               bulk_commit_group();
             }
           }
@@ -517,20 +545,29 @@ EncodeTiledFn get_encode_fn() {
 
 }  // namespace
 
-// 3-D bf16 tensor map: dims (inner, rows, batch); box (box_inner, box_rows, 1); SWIZZLE_128B.
-extern "C" int tepd_make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, long long inner, long long rows,
-                                      long long batch, long long ld_elems, long long batch_stride_elems,
-                                      int box_inner, int box_rows) {
+// 3-D tensor map of 2-byte (bf16) or 4-byte (fp32) elements: dims (inner, rows, batch); box (box_inner, box_rows, 1);
+// SWIZZLE_128B.
+static int make_tmap_3d(CUtensorMap* out, CUtensorMapDataType dtype, int elem_bytes, const void* ptr, long long inner,
+                        long long rows, long long batch, long long ld_elems, long long batch_stride_elems, int box_inner,
+                        int box_rows) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) return -1;
   cuuint64_t dims[3] = {(cuuint64_t)inner, (cuuint64_t)rows, (cuuint64_t)batch};
-  cuuint64_t strides[2] = {(cuuint64_t)ld_elems * 2, (cuuint64_t)(batch > 1 ? batch_stride_elems : rows * ld_elems) * 2};
+  cuuint64_t strides[2] = {(cuuint64_t)ld_elems * elem_bytes,
+                           (cuuint64_t)(batch > 1 ? batch_stride_elems : rows * ld_elems) * elem_bytes};
   cuuint32_t box[3] = {(cuuint32_t)box_inner, (cuuint32_t)box_rows, 1};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr,
+  CUresult r = fn(out, dtype, 3, const_cast<void*>(ptr), dims, strides, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : (int)r;
+}
+
+extern "C" int tepd_make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, long long inner, long long rows,
+                                      long long batch, long long ld_elems, long long batch_stride_elems,
+                                      int box_inner, int box_rows) {
+  return make_tmap_3d(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, inner, rows, batch, ld_elems, batch_stride_elems,
+                      box_inner, box_rows);
 }
 
 struct Maps { CUtensorMap a, b, d, d2, in; };
@@ -643,9 +680,12 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
   // Epilogue kind.  bf16 outputs go through shared memory and TMA when TMA can address the output and the residual / aux
   // (16-byte aligned base, row pitch and batch stride; aux and D2 share D's layout) and a staged kind exists for the
   // flags and the operand layout: plain for every layout, bias / bias + residual / dual GELU for the forward layout
-  // (A and B K-major), GELU' for the data-gradient layout (B MN-major).  Everything else stores from the fragments.
+  // (A and B K-major), GELU' for the data-gradient layout (B MN-major).  fp32 outputs of the weight-gradient layout (A and B
+  // MN-major) without bias, residual or activation go through shared memory too: plain stores, or TMA reduce-adds for
+  // accumulating outputs (split-K, stream-K, gradient accumulation); a stream-K fix-up of a plain store stays direct.
+  // Everything else stores from the fragments.
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  const bool fwd = !a_mn && !b_mn, dgrad = !a_mn && b_mn;
+  const bool fwd = !a_mn && !b_mn, dgrad = !a_mn && b_mn, wgrad = a_mn && b_mn;
   int epi = EPI_DIRECT;
   if (!out_fp32 && p.stream_k == 0 && ldd % 8 == 0 && (batch == 1 || stride_d % 8 == 0) && al16(D)) {
     const bool res_ok = residual != nullptr && al16(residual) && ld_res % 8 == 0 && (batch == 1 || stride_res % 8 == 0);
@@ -655,10 +695,16 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
     else if (act == 1 && D2 && al16(D2) && !residual && fwd) epi = EPI_GELU_DUAL;
     else if (act == 2 && al16(aux) && !bias && !residual && dgrad) epi = EPI_GELU_BWD;
   }
+  if (out_fp32 && wgrad && act == 0 && !bias && !residual && (accumulate || p.stream_k == 0) && ldd % 4 == 0 &&
+      (batch == 1 || stride_d % 4 == 0) && al16(D))
+    epi = accumulate ? EPI_F32_ADD : EPI_F32;
   Maps m;
   m.a = ta; m.b = tb;
   m.d = m.d2 = m.in = CUtensorMap{};
-  if (epi != EPI_DIRECT) {
+  if (epi == EPI_F32 || epi == EPI_F32_ADD) {
+    rc = make_tmap_3d(&m.d, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, D, N, M, batch, ldd, stride_d, STORE_BOX_F32, 64);
+    if (rc) return 300 + rc;
+  } else if (epi != EPI_DIRECT) {
     rc = tepd_make_tmap_bf16_3d(&m.d, D, N, M, batch, ldd, stride_d, STORE_BOX, 64);
     if (!rc && epi == EPI_GELU_DUAL) rc = tepd_make_tmap_bf16_3d(&m.d2, D2, N, M, batch, ldd, stride_d, STORE_BOX, 64);
     if (!rc && epi == EPI_BIAS_RES) rc = tepd_make_tmap_bf16_3d(&m.in, residual, N, M, batch, ld_res, stride_res, STORE_BOX, 64);
@@ -678,6 +724,8 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
     case EPI_BIAS_RES: return launch_gemm<BN, false, false, false, EPI_BIAS_RES>(m, p, num_sms, s);       \
     case EPI_GELU_DUAL: return launch_gemm<BN, false, false, false, EPI_GELU_DUAL>(m, p, num_sms, s);     \
     case EPI_GELU_BWD: return launch_gemm<BN, false, true, false, EPI_GELU_BWD>(m, p, num_sms, s);        \
+    case EPI_F32: return launch_gemm<BN, true, true, false, EPI_F32>(m, p, num_sms, s);                   \
+    case EPI_F32_ADD: return launch_gemm<BN, true, true, false, EPI_F32_ADD>(m, p, num_sms, s);           \
     default: { LAYOUTS(BN, EPI_DIRECT) }                                                                  \
   }
   if (block_n == 256) { KINDS(256) } else { KINDS(128) }

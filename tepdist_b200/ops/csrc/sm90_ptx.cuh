@@ -118,6 +118,12 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* s
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
+// The same box, added element-wise into global memory (fp32 add at L2; also a bulk-group operation, also clipped).
+__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // wait until at most N committed bulk groups still read their shared-memory source / are still in flight at all
 template <int N>
