@@ -1,14 +1,14 @@
 // Fused (flash) attention for sm_90a, head_dim 64 or 128, bf16, with wgmma.mma_async on register accumulators.
-// Forward, one CTA per (128-query block, batch, head): two warpgroups own 64 query rows each, a producer (one warp at
-// D = 64, a warpgroup at D = 128) streams K / V tiles through a TMA + mbarrier ring.
+// Forward, one CTA per (128-query block, batch, head): two warpgroups own 64 query rows each, a producer warpgroup streams
+// K / V tiles through a TMA + mbarrier ring.
 //   S = Q K^T            wgmma m64n128k16 (A = Q, B = K, both K-major in smem)        -> registers
 //   P = online softmax   in registers (quad shuffles for the row max / sum)
 //   O += P V             wgmma m64nDk16 with A = P from registers (the S fragment repacked to bf16), B = V MN-major
 // Q/K/V are read straight out of the fused qkv projection buffer [B, S, H, 3, D] (heads-major) with 4-D TMA maps
 // (no head-split transposes), O is written as [B, S, H, D] so it feeds the output projection GEMM.
 // A D-wide row tile is D / 64 SW128 column chunks of [rows x 64] (128 B per row), each loaded by one TMA box.
-// At D = 128 the O (fwd) and dK + dV (bwd) accumulators double: the producer warpgroup drops to 24 registers with
-// setmaxnreg and the two consumer warpgroups take 240 each, so neither kernel spills.
+// The producer warpgroup drops to 24 registers with setmaxnreg and the two consumer warpgroups take 240 each, so no kernel
+// spills even where the O (fwd) and dK + dV (bwd) accumulators double at D = 128.
 // The reference gets attention from XLA-fused batched dots + softmax fusions (SURVEY Appendix C);
 // this kernel is the H100-native replacement.
 #include "sm90_ptx.cuh"
@@ -28,7 +28,7 @@ template <int HD>
 struct AttnCfg;
 template <>
 struct AttnCfg<64> {
-  static constexpr int THREADS = 288;  // warps 0..7: two compute warpgroups, warp 8: TMA producer
+  static constexpr int THREADS = 384;  // warpgroups 0, 1: compute (240 registers), warpgroup 2: TMA producer (24)
   static constexpr int KV_STAGES = 3;
   static constexpr int Q_STAGES = 3;
 };
@@ -103,9 +103,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
   int j0 = 0;   // first KV tile (stage and phase indices count from it)
   if constexpr (DOC) j0 = __ldg(p.doc_start + (size_t)b * p.S + qi * BQ) / BKV;
 
-  if (HD == 64 ? warp == 8 : warp >= 8) {   // producer: warp 8 (D = 64) / warpgroup 2 (D = 128)
-    if constexpr (HD == 128) setmaxnreg_dec<24>();
-    if (lane == 0 && (HD == 64 || warp == 8)) {
+  if (warp >= 8) {   // producer warpgroup
+    setmaxnreg_dec<24>();
+    if (lane == 0 && warp == 8) {
       mbar_expect_tx(q_full, L::TILE_BYTES);
 #pragma unroll
       for (int c = 0; c < NC; ++c) tma_load_4d(smem + L::SM_Q + c * CHUNK, &tmap_q, q_full, c * 64, qi * BQ, h, b);
@@ -124,7 +124,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     pdl_trigger();
     return;
   }
-  if constexpr (HD == 128) setmaxnreg_inc<240>();
+  setmaxnreg_inc<240>();
 
   const int wg = warp >> 2;
   const int g = lane >> 2, q = lane & 3;
@@ -141,20 +141,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     ds[1] = __ldg(dsb + row0 + 8);
     ds_last = __ldg(dsb + BQ - 1);
   }
-  mbar_wait(q_full, 0);
-  for (int j = j0; j < nkv; ++j) {
-    const int st = (j - j0) % KV_STAGES;
-    mbar_wait(&kv_full[st], ((j - j0) / KV_STAGES) & 1);
-    const uint32_t sk = smem_u32(smem + L::SM_K + st * L::TILE_BYTES), sv = smem_u32(smem + L::SM_V + st * L::TILE_BYTES);
-    float s[64];
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < HD / 16; ++k)
-      wgmma_m64n128k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sq + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024),
-                                     make_smem_desc_sw128(sk + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024), k > 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(s);
+  // online softmax of the score tile of KV tile j: s -> P (fp32), running max / sum updated, alpha = the factor O is rescaled by
+  auto softmax = [&](float (&s)[64], int j, float (&alpha)[2]) {
     const bool diag = p.causal && j == qi;
     if (DOC && j * BKV < ds_last) {   // some key of this tile lies before the document start of some row (a separate pass:
                                       // the tiles without one run the plain softmax)
@@ -183,7 +171,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
       // safe max: a row that has seen only masked keys keeps m = -inf, and subtracting 0 instead gives p = 0, alpha = 0
       const float mxs = DOC && mx == -INFINITY ? 0.f : mx;
-      const float alpha = exp2f(m[hr] - mxs);
+      alpha[hr] = exp2f(m[hr] - mxs);
       m[hr] = mx;
       float sum = 0.f;
 #pragma unroll
@@ -196,25 +184,155 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           sum += pv;
         }
       }
-      l[hr] = l[hr] * alpha + sum;
+      l[hr] = l[hr] * alpha[hr] + sum;
+    }
+  };
+  auto rescale_o = [&](const float (&alpha)[2]) {
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr)
 #pragma unroll
       for (int jj = 0; jj < HD / 8; ++jj) {
-        o[4 * jj + 2 * hr] *= alpha;
-        o[4 * jj + 2 * hr + 1] *= alpha;
+        o[4 * jj + 2 * hr] *= alpha[hr];
+        o[4 * jj + 2 * hr + 1] *= alpha[hr];
       }
-    }
+  };
+  auto issue_s = [&](float (&s)[64], int j) {   // S = Q K_j^T (one commit group)
+    const int st = (j - j0) % KV_STAGES;
+    mbar_wait(&kv_full[st], ((j - j0) / KV_STAGES) & 1);
+    const uint32_t sk = smem_u32(smem + L::SM_K + st * L::TILE_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < HD / 16; ++k)
+      wgmma_m64n128k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sq + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024),
+                                     make_smem_desc_sw128(sk + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024), k > 0 ? 1u : 0u);
+    wgmma_commit();
+  };
+  auto issue_pv = [&](const uint32_t (&pa)[32], int j) {   // O += P V_j (one commit group); P packed to bf16 A fragments
+    const uint32_t sv = smem_u32(smem + L::SM_V + ((j - j0) % KV_STAGES) * L::TILE_BYTES);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < 8; ++kk) {
-      uint32_t a[4];
-      frag_a_from_acc(s, kk, a);
+      const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
       // V MN-major: LBO = the next 64-column chunk (the field is unused at N = 64)
       wgmma_m64nXk16_bf16_rs<1>(o, a, make_smem_desc_sw128(sv + kk * 16 * 128, HD == 64 ? 8192 : CHUNK, 1024), 1u);
     }
     wgmma_commit();
+  };
+  auto pack_p = [&](const float (&s)[64], uint32_t (&pa)[32]) {
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      uint32_t a[4];
+      frag_a_from_acc(s, kk, a);
+#pragma unroll
+      for (int t = 0; t < 4; ++t) pa[4 * kk + t] = a[t];
+    }
+  };
+  auto release = [&](int j) {
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[(j - j0) % KV_STAGES]);
+  };
+  mbar_wait(q_full, 0);
+  if constexpr (HD == 64) {
+    // Software-pipelined: S_{j+1} = Q K_{j+1}^T and O += P_j V_j are in flight while the softmax of S_{j+1} runs; O is
+    // rescaled once P_j V_j has landed, so every tile sees the same arithmetic in the same order as the unpipelined loop.
+    float s[64], alpha[2];
+    uint32_t pa[32];
+    issue_s(s, j0);
+    wgmma_wait<0>();
+    fence_regs(s);
+    softmax(s, j0, alpha);
+    rescale_o(alpha);
+    pack_p(s, pa);
+    for (int j = j0 + 1; j < nkv; ++j) {
+      issue_s(s, j);
+      issue_pv(pa, j - 1);
+      wgmma_wait<1>();
+      fence_regs(s);
+      softmax(s, j, alpha);
+      wgmma_wait<0>();
+      fence_regs(o);
+      release(j - 1);
+      rescale_o(alpha);
+      pack_p(s, pa);
+    }
+    issue_pv(pa, nkv - 1);
     wgmma_wait<0>();
     fence_regs(o);
-    if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[st]);
+    release(nkv - 1);
+  } else {
+    for (int j = j0; j < nkv; ++j) {
+      const int st = (j - j0) % KV_STAGES;
+      mbar_wait(&kv_full[st], ((j - j0) / KV_STAGES) & 1);
+      const uint32_t sk = smem_u32(smem + L::SM_K + st * L::TILE_BYTES), sv = smem_u32(smem + L::SM_V + st * L::TILE_BYTES);
+      float s[64];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < HD / 16; ++k)
+        wgmma_m64n128k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sq + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024),
+                                       make_smem_desc_sw128(sk + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024), k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+      const bool diag = p.causal && j == qi;
+      if (DOC && j * BKV < ds_last) {   // some key of this tile lies before the document start of some row (a separate pass:
+                                        // the tiles without one run the plain softmax)
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            if (j * BKV + 8 * jj + 2 * q + (e & 1) < ds[e >> 1]) s[4 * jj + e] = -INFINITY;
+      }
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int r = row0 + hr * 8;
+        float mx = m[hr];
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int idx = 4 * jj + 2 * hr + e;
+            float x = s[idx] * p.scale_log2;
+            if (diag && 8 * jj + 2 * q + e > r) x = -INFINITY;
+            s[idx] = x;
+            mx = fmaxf(mx, x);
+          }
+        }
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        // safe max: a row that has seen only masked keys keeps m = -inf, and subtracting 0 instead gives p = 0, alpha = 0
+        const float mxs = DOC && mx == -INFINITY ? 0.f : mx;
+        const float alpha = exp2f(m[hr] - mxs);
+        m[hr] = mx;
+        float sum = 0.f;
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int idx = 4 * jj + 2 * hr + e;
+            const float pv = exp2f(s[idx] - mxs);
+            s[idx] = pv;
+            sum += pv;
+          }
+        }
+        l[hr] = l[hr] * alpha + sum;
+#pragma unroll
+        for (int jj = 0; jj < HD / 8; ++jj) {
+          o[4 * jj + 2 * hr] *= alpha;
+          o[4 * jj + 2 * hr + 1] *= alpha;
+        }
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        uint32_t a[4];
+        frag_a_from_acc(s, kk, a);
+        // V MN-major: LBO = the next 64-column chunk (the field is unused at N = 64)
+        wgmma_m64nXk16_bf16_rs<1>(o, a, make_smem_desc_sw128(sv + kk * 16 * 128, HD == 64 ? 8192 : CHUNK, 1024), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(o);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&kv_empty[st]);
+    }
   }
   pdl_trigger();
 #pragma unroll
@@ -239,18 +357,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 //   P^T = exp2(S^T c - lse), dS^T = P^T (dP^T - delta)          in registers
 //   dV += P^T dO, dK += dS^T Q                      wgmma m64nDk16 with A from registers, B (dO / Q) MN-major in smem
 //   dQ  = dS K over this warpgroup's 64 kv rows      dS^T goes through smem (read as an MN-major A operand) ->
-//                                                   fp32 red.add into dq_acc (summed over kv blocks / warpgroups),
-//                                                   one 64-column half of D at a time (keeps D = 128 within 240 registers)
+//                                                   summed into dq_acc over kv blocks / warpgroups: at D = 128 by fp32
+//                                                   red.add from the fragments, one 64-column half of D at a time (keeps
+//                                                   it within 240 registers); at D = 64 staged in smem and added by one
+//                                                   bulk reduce-add per warpgroup and block
+// At D = 64 lse / delta come from smem (bulk-copied by the producer with each Q / dO stage), S^T and dP^T are separate
+// commit groups, and dV += P^T dO runs while dS^T is formed.
 // =====================================================================================================
 constexpr int BQB = 64;                          // query rows per backward iteration
-
-// The backward's producer is a whole warpgroup that hands its registers to the consumers (setmaxnreg) at D = 128, and also
-// for the document-masked D = 64 kernel, whose extra masking state would otherwise spill under the 288-thread layout.
-template <int HD, bool DOC>
-struct BwdLayout {
-  static constexpr bool WG_PRODUCER = HD == 128 || DOC;
-  static constexpr int THREADS = WG_PRODUCER ? 384 : AttnCfg<HD>::THREADS;
-};
 
 template <int HD>
 struct BwdSmem {
@@ -263,14 +377,19 @@ struct BwdSmem {
   static constexpr int SB_DS = SB_V + KV_BYTES;
   static constexpr int SB_Q = SB_DS + DS_BYTES;   // [Q_STAGES]
   static constexpr int SB_DO = SB_Q + AttnCfg<HD>::Q_STAGES * QB_BYTES;
-  static constexpr int SB_BAR = SB_DO + AttnCfg<HD>::Q_STAGES * QB_BYTES;
+  // D = 64 only: each warpgroup's fp32 [64 q x 64] dQ partial, and per Q / dO stage the block's 64 lse + 64 delta values
+  static constexpr int DQ_BYTES = HD == 64 ? BQB * 64 * 4 : 0;
+  static constexpr int STAT_BYTES = HD == 64 ? 2 * BQB * 4 : 0;
+  static constexpr int SB_DQ = SB_DO + AttnCfg<HD>::Q_STAGES * QB_BYTES;   // [2 warpgroups]
+  static constexpr int SB_STAT = SB_DQ + 2 * DQ_BYTES;                     // [Q_STAGES]
+  static constexpr int SB_BAR = SB_STAT + AttnCfg<HD>::Q_STAGES * STAT_BYTES;
   static constexpr int BYTES = SB_BAR + 256 + 1024;
 };
 
 struct AttnBwdParams {
   const float* lse;    // [B,H,S]
   const float* delta;  // [B,H,S]
-  float* dq_acc;       // fp32 [B,S,H,D] (zero-initialised)
+  float* dq_acc;       // fp32, zero-initialised: [B, S, H, 128] at D = 128, [B, H, S, 64] (see attn_dq_cast_kernel) at D = 64
   void* dk;            // bf16, strided [B,S,H,D] view
   void* dv;
   long long dstride_b, dstride_s, dstride_h;
@@ -284,7 +403,7 @@ struct AttnBwdParams {
 // monotone, those queries are a suffix for each key row, so a thread keeps one bound per kv row instead of loading
 // doc_start per query column.
 template <int HD, bool DOC>
-__global__ void __launch_bounds__(BwdLayout<HD, DOC>::THREADS, 1)
+__global__ void __launch_bounds__(AttnCfg<HD>::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
                 const AttnBwdParams p) {
@@ -332,9 +451,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     }
   }
 
-  constexpr bool WGP = BwdLayout<HD, DOC>::WG_PRODUCER;
-  if (WGP ? warp >= 8 : warp == 8) {   // producer: warpgroup 2 (setmaxnreg) / warp 8
-    if constexpr (WGP) setmaxnreg_dec<24>();
+  if (warp >= 8) {   // producer warpgroup
+    setmaxnreg_dec<24>();
     if (lane == 0 && warp == 8) {
       mbar_expect_tx(kv_full, 2 * L::KV_BYTES);
 #pragma unroll
@@ -344,7 +462,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       for (int i = i0, it = 0; i < i_end; ++i, ++it) {
         const int st = it % Q_STAGES;
         mbar_wait(&q_empty[st], ((it / Q_STAGES) & 1) ^ 1);
-        mbar_expect_tx(&q_full[st], 2 * L::QB_BYTES);
+        mbar_expect_tx(&q_full[st], 2 * L::QB_BYTES + L::STAT_BYTES);
+        if constexpr (HD == 64) {
+          float* stat = reinterpret_cast<float*>(smem + L::SB_STAT + st * L::STAT_BYTES);
+          const size_t row = ((size_t)b * p.H + h) * p.S + i * BQB;
+          bulk_load(stat, p.lse + row, BQB * 4, &q_full[st]);
+          bulk_load(stat + BQB, p.delta + row, BQB * 4, &q_full[st]);
+        }
 #pragma unroll
         for (int c = 0; c < NC; ++c)
           tma_load_4d(smem + L::SB_Q + st * L::QB_BYTES + c * L::QB_CHUNK, &tmap_q, &q_full[st], c * 64, i * BQB, h, b);
@@ -356,7 +480,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     pdl_trigger();
     return;
   }
-  if constexpr (WGP) setmaxnreg_inc<240>();
+  setmaxnreg_inc<240>();
 
   const int wg = warp >> 2;
   const int g = lane >> 2, q = lane & 3;
@@ -394,16 +518,61 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     for (int k = 0; k < HD / 16; ++k)
       wgmma_m64n64k16_bf16_ss<0, 0>(s, make_smem_desc_sw128(sk + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024),
                                     make_smem_desc_sw128(sq + (k / 4) * L::QB_CHUNK + (k % 4) * 32, 0, 1024), k > 0 ? 1u : 0u);
+    if constexpr (HD == 64) wgmma_commit();   // S^T and dP^T in separate groups: P^T is computed while dP^T runs
 #pragma unroll
     for (int k = 0; k < HD / 16; ++k)
       wgmma_m64n64k16_bf16_ss<0, 0>(dp, make_smem_desc_sw128(sv + (k / 4) * CHUNK + (k % 4) * 32, 0, 1024),
                                     make_smem_desc_sw128(sdo + (k / 4) * L::QB_CHUNK + (k % 4) * 32, 0, 1024), k > 0 ? 1u : 0u);
     wgmma_commit();
+    const bool masked = p.causal && i * BQB < j * BKV + BKV;   // query block overlaps the kv block
+    const bool dmask = DOC && i * BQB + BQB > min(qend[0], qend[1]);   // some query of the block is past a kv row's document
+    if constexpr (HD == 64) {
+      const float* stat = reinterpret_cast<const float*>(smem + L::SB_STAT + st * L::STAT_BYTES);
+      wgmma_wait<1>();
+      fence_regs(s);
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+        for (int e1 = 0; e1 < 2; ++e1) {
+          const int qt = 8 * jj + 2 * q + e1;
+          const float L2 = stat[qt] * 1.4426950408889634f;
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            const int idx = 4 * jj + 2 * hr + e1;
+            float pv = exp2f(s[idx] * p.scale_log2 - L2);
+            if (masked && i * BQB + qt < j * BKV + wg * 64 + r0 + 8 * hr) pv = 0.f;
+            if (dmask && i * BQB + qt >= qend[hr]) pv = 0.f;
+            s[idx] = pv;
+          }
+        }
+      }
+      // dV += P^T dO runs while dS^T is formed
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        uint32_t a[4];
+        frag_a_from_acc(s, kk, a);
+        wgmma_m64nXk16_bf16_rs<1>(dv, a, make_smem_desc_sw128(sdo + kk * 16 * 128, L::QB_CHUNK, 1024), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      fence_regs(dp);
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+        for (int e1 = 0; e1 < 2; ++e1) {
+          const float dl = stat[BQB + 8 * jj + 2 * q + e1];
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr) {
+            const int idx = 4 * jj + 2 * hr + e1;
+            dp[idx] = s[idx] * (dp[idx] - dl);
+          }
+        }
+      }
+    } else {
     wgmma_wait<0>();
     fence_regs(s);
     fence_regs(dp);
-    const bool masked = p.causal && i * BQB < j * BKV + BKV;   // query block overlaps the kv block
-    const bool dmask = DOC && i * BQB + BQB > min(qend[0], qend[1]);   // some query of the block is past a kv row's document
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
@@ -422,7 +591,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         }
       }
     }
+    }
     // dS^T -> smem: element (kv row r, query column c) at byte r * 128 + 2c of the SW128 tile (16-byte chunk index XOR r % 8)
+    if (HD == 64 && (threadIdx.x & 127) == 0) bulk_wait_group_read<0>();   // the last dQ reduce has read its partial
     named_bar_sync(1 + wg, 128);   // this warpgroup's previous dQ MMA has finished reading the tile
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
@@ -437,11 +608,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     named_bar_sync(1 + wg, 128);
     wgmma_fence();
     // dO / Q MN-major: LBO = the next 64-column chunk (the field is unused at N = 64)
+    if constexpr (HD == 128) {
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
       uint32_t a[4];
       frag_a_from_acc(s, kk, a);
       wgmma_m64nXk16_bf16_rs<1>(dv, a, make_smem_desc_sw128(sdo + kk * 16 * 128, L::QB_CHUNK, 1024), 1u);
+    }
     }
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
@@ -465,6 +638,25 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       }
       fence_regs(dq);
       if (n == 0 && (threadIdx.x & 127) == 0) mbar_arrive(&q_empty[st]);
+      if constexpr (HD == 64) {
+        // the warpgroup's [64 q x 64] partial -> smem (8-column groups XOR row % 4: conflict-free float2 stores), one bulk
+        // reduce-add of the contiguous 16 KB block into dq_acc [B, H, S, 64]
+        float* dq_tile = reinterpret_cast<float*>(smem + L::SB_DQ + wg * L::DQ_BYTES);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const int r = r0 + 8 * hr;
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj)
+            *reinterpret_cast<float2*>(dq_tile + r * 64 + 8 * (jj ^ (r & 3)) + 2 * q) =
+                make_float2(dq[4 * jj + 2 * hr] * p.scale, dq[4 * jj + 2 * hr + 1] * p.scale);
+        }
+        fence_proxy_async();
+        named_bar_sync(1 + wg, 128);
+        if ((threadIdx.x & 127) == 0) {
+          bulk_reduce_add_f32(p.dq_acc + (((size_t)b * p.H + h) * p.S + i * BQB) * 64, dq_tile, L::DQ_BYTES);
+          bulk_commit_group();
+        }
+      } else {
 #pragma unroll
       for (int hr = 0; hr < 2; ++hr) {
         const int row = i * BQB + r0 + 8 * hr;
@@ -475,9 +667,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
                        "f"(dq[4 * jj + 2 * hr + 1] * p.scale)
                        : "memory");
       }
+      }
     }
   }
   pdl_trigger();
+  if (HD == 64 && (threadIdx.x & 127) == 0) bulk_wait_group<0>();   // the dQ partials live until the last reduce is done
 #pragma unroll
   for (int hr = 0; hr < 2; ++hr) {
     const int row = j * BKV + wg * 64 + r0 + 8 * hr;
@@ -519,7 +713,8 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ dO, const __
   if (sub == 0) delta[((size_t)bb * H + hh) * S + s] = v;
 }
 
-// dq (bf16, strided) = dq_acc (fp32 contiguous [B,S,H,D])
+// dq (bf16, strided) = dq_acc, fp32 contiguous: [B, S, H, 128] at D = 128; [B, H, S, 64] at D = 64, with the 8-column
+// groups of row s stored at group index (v ^ s % 4) (the layout the backward's bulk reduce-adds write).
 // (the accumulator is zeroed again on the way out, so the persistent workspace never needs a separate memset)
 template <int HD>
 __global__ void attn_dq_cast_kernel(float* __restrict__ acc, __nv_bfloat16* __restrict__ dq, int B, int S, int H,
@@ -532,12 +727,13 @@ __global__ void attn_dq_cast_kernel(float* __restrict__ acc, __nv_bfloat16* __re
     const int hh = r % H; r /= H;
     const int s = r % S;
     const int bb = r / S;
-    const float4 x = reinterpret_cast<const float4*>(acc)[i * 2], y = reinterpret_cast<const float4*>(acc)[i * 2 + 1];
+    const size_t a = HD == 64 ? (((size_t)bb * H + hh) * S + s) * 8 + (v ^ (s & 3)) : i;   // 8-float group in acc
+    const float4 x = reinterpret_cast<const float4*>(acc)[a * 2], y = reinterpret_cast<const float4*>(acc)[a * 2 + 1];
     uint4 u;
     u.x = pack_bf16x2(x.x, x.y); u.y = pack_bf16x2(x.z, x.w); u.z = pack_bf16x2(y.x, y.y); u.w = pack_bf16x2(y.z, y.w);
     *reinterpret_cast<uint4*>(dq + (size_t)bb * sb + (size_t)s * ss + (size_t)hh * sh + v * 8) = u;
-    reinterpret_cast<float4*>(acc)[i * 2] = make_float4(0.f, 0.f, 0.f, 0.f);
-    reinterpret_cast<float4*>(acc)[i * 2 + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
+    reinterpret_cast<float4*>(acc)[a * 2] = make_float4(0.f, 0.f, 0.f, 0.f);
+    reinterpret_cast<float4*>(acc)[a * 2 + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
 
@@ -637,8 +833,7 @@ int attn_bwd(const void* dO, const void* q, const void* k, const void* v, const 
   p.dstride_b = dstride_b; p.dstride_s = dstride_s; p.dstride_h = dstride_h;
   p.B = B; p.H = H; p.S = S; p.causal = causal; p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   p.doc_start = doc_start;
-  const int threads = doc_start ? BwdLayout<HD, true>::THREADS : BwdLayout<HD, false>::THREADS;
-  cudaError_t le = tepd::launch(kern, dim3((S / BKV) * B * H), dim3(threads), BwdSmem<HD>::BYTES, st,
+  cudaError_t le = tepd::launch(kern, dim3((S / BKV) * B * H), dim3(AttnCfg<HD>::THREADS), BwdSmem<HD>::BYTES, st,
                                 tq, tk, tv, tdo, p);
   if (le != cudaSuccess) return (int)le;
   return (int)tepd::launch(attn_dq_cast_kernel<HD>, dim3(tepd::num_sms() * 4), dim3(256), 0, st, dq_acc, (__nv_bfloat16*)dq, B, S,
@@ -660,11 +855,14 @@ extern "C" int tepd_attn_fwd(const void* q, const void* k, const void* v, void* 
 }
 
 // do, o: contiguous [B,S,H,D]; q/k/v strided views; dq/dk/dv strided views (shared strides).  D = 64 or 128.
+// lse: contiguous fp32 [B, H, S] (16-byte aligned at D = 64).  dq_acc: nullptr (a persistent, self-clearing workspace of the
+// library's) or a zeroed fp32 buffer of B * S * H * D elements in the layout attn_dq_cast_kernel reads; left zeroed.
 extern "C" int tepd_attn_bwd(const void* dO, const void* q, const void* k, const void* v, const void* o, const void* lse,
                              void* dq_acc, void* dq, void* dk, void* dv, int B, int H, int S, int D, float scale,
                              int causal, long long stride_b, long long stride_s, long long stride_h, long long dstride_b,
                              long long dstride_s, long long dstride_h, void* stream, const int* doc_start) {
   if ((D != 64 && D != 128) || S % 128 != 0 || (doc_start && !causal)) return -2;
+  if (D == 64 && (reinterpret_cast<uintptr_t>(lse) & 15)) return -2;   // lse rows are bulk-copied (16-byte alignment)
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   static float* delta_buf = nullptr;
   static size_t delta_cap = 0;

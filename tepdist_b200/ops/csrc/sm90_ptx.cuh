@@ -124,6 +124,18 @@ __device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, const vo
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
+// Non-tensor bulk copies (contiguous bytes; addresses and size multiples of 16): global -> shared on an mbarrier, and a
+// shared -> global fp32 element-wise add (bulk-group completion).
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+__device__ __forceinline__ void bulk_reduce_add_f32(float* dst, const void* smem_src, uint32_t bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;"
+               ::"l"(reinterpret_cast<uint64_t>(dst)), "r"(smem_u32(smem_src)), "r"(bytes)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // wait until at most N committed bulk groups still read their shared-memory source / are still in flight at all
 template <int N>
