@@ -87,6 +87,8 @@ class _Sig:
     tepd_bn_reduce_nhwc = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]
     tepd_bn_fwd_apply_nhwc = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _i, _f, _vp]
     tepd_bn_bwd_apply_nhwc = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp]
+    tepd_bn_centred_sq_nhwc = [_vp, _vp, _i, _i, _f, _vp]
+    tepd_bn_fwd_apply_centred_nhwc = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _i, _f, _vp]
     tepd_im2col_nhwc = [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]
     tepd_col2im_nhwc = [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]
     tepd_embedding_fwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]
@@ -557,7 +559,7 @@ def batchnorm_fwd(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps:
     rstd = torch.empty(C, dtype=torch.float32, device=x.device)
     _check(lib().tepd_bn_fwd_nhwc(xn.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
                                   ws.data_ptr(), N * H * W, C, float(eps), int(relu), _stream()), "bn_fwd")
-    _count(2)
+    _count(3)
     return y.permute(0, 3, 1, 2), mean, rstd
 
 
@@ -575,20 +577,25 @@ def batchnorm_bwd(dy: torch.Tensor, x: torch.Tensor, gamma: torch.Tensor, mean: 
 
 def batchnorm_fwd_synced(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, allsum, num_shards: int,
                          relu: bool = False):
-    """Synchronised training-mode BatchNorm, native split phases: local per-channel sums (bn_reduce2), `allsum(ws)` completes them
-    over the devices that split the batch (one all-reduce of 2 x C floats), apply with the GLOBAL count.  -> (y, mean, rstd)."""
+    """Synchronised training-mode BatchNorm, native split phases with the same two-pass statistics as one device: local
+    sum(x), `allsum(ws[0])` completes it over the devices that split the batch; local sum((x - mean)^2) around that global
+    mean, `allsum(ws[1])`; apply with the GLOBAL count.  Two all-reduces of C floats.  -> (y, mean, rstd)."""
     N, C, H, W = x.shape
     xn = _nhwc(x)
     rows = N * H * W
+    count = float(rows * num_shards)
     y = torch.empty_like(xn)
     ws = torch.zeros(2, C, dtype=torch.float32, device=x.device)
     mean = torch.empty(C, dtype=torch.float32, device=x.device)
     rstd = torch.empty(C, dtype=torch.float32, device=x.device)
-    _check(lib().tepd_bn_reduce_nhwc(xn.data_ptr(), None, None, None, ws.data_ptr(), rows, C, 0, _stream()), "bn_reduce")
-    allsum(ws)
-    _check(lib().tepd_bn_fwd_apply_nhwc(xn.data_ptr(), ws.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(), mean.data_ptr(),
-                                        rstd.data_ptr(), rows, C, float(eps), int(relu), float(rows * num_shards), _stream()), "bn_fwd_apply")
-    _count(2)
+    _check(lib().tepd_bn_reduce_nhwc(xn.data_ptr(), None, None, None, ws.data_ptr(), rows, C, 2, _stream()), "bn_reduce")
+    allsum(ws[0])
+    _check(lib().tepd_bn_centred_sq_nhwc(xn.data_ptr(), ws.data_ptr(), rows, C, count, _stream()), "bn_centred_sq")
+    allsum(ws[1])
+    _check(lib().tepd_bn_fwd_apply_centred_nhwc(xn.data_ptr(), ws.data_ptr(), gamma.data_ptr(), beta.data_ptr(), y.data_ptr(),
+                                                mean.data_ptr(), rstd.data_ptr(), rows, C, float(eps), int(relu), count, _stream()),
+           "bn_fwd_apply")
+    _count(3)
     return y.permute(0, 3, 1, 2), mean, rstd
 
 

@@ -240,17 +240,21 @@ __global__ void gelu_bwd_kernel(const uint4* __restrict__ dy, const uint4* __res
 }
 
 // ------------------------------------------------------------------ BatchNorm (training mode) on NHWC rows
-// x is [rows = N*H*W, C] (channels_last memory).  Two passes each way, both column-parallel like colsum:
-//   forward : bn_reduce2 accumulates sum(x) and sum(x^2) per channel (fp32 atomics over row strips), bn_fwd_apply turns
-//             them into mean / rstd and writes y = (x - mean) * rstd * gamma + beta (+ ReLU);
+// x is [rows = N*H*W, C] (channels_last memory).  All passes are column-parallel like colsum:
+//   forward : bn_reduce2 accumulates sum(x) per channel (fp32 atomics over row strips), then the centred second moment
+//             sum((x - mean)^2) with mean = sum(x) / count; bn_fwd_apply<true> turns them into mean / rstd and writes
+//             y = (x - mean) * rstd * gamma + beta (+ ReLU).  The one-pass form E[x^2] - E[x]^2 (MODE 0, apply<false>) loses
+//             all of its digits when |mean| >> std (a channel at mean / std = 300 keeps none of them in fp32), so the
+//             library's own forward no longer uses it; it stays behind the split-phase mode 0 for existing callers.
 //   backward: bn_reduce2 with dy accumulates sum(dy) and sum(dy * xhat), bn_bwd_apply writes
 //             dx = gamma * rstd * (dy - mean(dy) - xhat * mean(dy * xhat)).
-// MODE 0: (x, x^2); MODE 1: (dy, dy * xhat) with xhat recomputed from x, mean, rstd.
+// MODE 0: (x, x^2); MODE 1: (dy, dy * xhat) with xhat recomputed from x, mean, rstd; MODE 2: x into out0 only;
+// MODE 3: (x - mu)^2 into out1 only, mu = out0 / count computed exactly as bn_fwd_apply computes it (out0 is only read).
 template <int MODE>
 __global__ void __launch_bounds__(256) bn_reduce2_kernel(const bf16* __restrict__ a, const bf16* __restrict__ x,
                                                         const float* __restrict__ mean, const float* __restrict__ rstd,
                                                         float* __restrict__ out0, float* __restrict__ out1, int rows, int C,
-                                                        int rows_per_block) {
+                                                        int rows_per_block, float count) {
   __shared__ float red[2][8][256];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int col0 = blockIdx.x * 256 + lane * 8;
@@ -264,12 +268,23 @@ __global__ void __launch_bounds__(256) bn_reduce2_kernel(const bf16* __restrict_
 #pragma unroll
       for (int j = 0; j < 8; ++j) { mu[j] = mean[col0 + j]; rs[j] = rstd[col0 + j]; }
     }
+    if (MODE == 3) {
+      const float inv = 1.f / count;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) mu[j] = out0[col0 + j] * inv;
+    }
     for (int r = r0 + warp; r < r1; r += 8) {
       float f[8];
       unpack8(__ldg(reinterpret_cast<const uint4*>(a + (size_t)r * C + col0)), f);
       if (MODE == 0) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) { s0[j] += f[j]; s1[j] += f[j] * f[j]; }
+      } else if (MODE == 2) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) s0[j] += f[j];
+      } else if (MODE == 3) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { const float d = f[j] - mu[j]; s1[j] += d * d; }
       } else {
         float xv[8];
         unpack8(__ldg(reinterpret_cast<const uint4*>(x + (size_t)r * C + col0)), xv);
@@ -286,12 +301,13 @@ __global__ void __launch_bounds__(256) bn_reduce2_kernel(const bf16* __restrict_
     float t0 = 0.f, t1 = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) { t0 += red[0][w][c]; t1 += red[1][w][c]; }
-    atomicAdd(out0 + blockIdx.x * 256 + c, t0);
-    atomicAdd(out1 + blockIdx.x * 256 + c, t1);
+    if (MODE != 3) atomicAdd(out0 + blockIdx.x * 256 + c, t0);
+    if (MODE != 2) atomicAdd(out1 + blockIdx.x * 256 + c, t1);
   }
 }
 
-// sums = [sum(x), sum(x^2)] -> mean, rstd (written by block row 0) and y
+// CENTRED: sums = [sum(x), sum((x - mean)^2)], else [sum(x), sum(x^2)] -> mean, rstd (written by block row 0) and y
+template <bool CENTRED>
 __global__ void __launch_bounds__(256) bn_fwd_apply_kernel(const bf16* __restrict__ x, const float* __restrict__ sum,
                                                           const float* __restrict__ sumsq, const float* __restrict__ gamma,
                                                           const float* __restrict__ beta, bf16* __restrict__ y,
@@ -307,7 +323,7 @@ __global__ void __launch_bounds__(256) bn_fwd_apply_kernel(const bf16* __restric
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float mu = sum[c0 + j] * inv;
-      const float var = fmaxf(sumsq[c0 + j] * inv - mu * mu, 0.f);
+      const float var = CENTRED ? sumsq[c0 + j] * inv : fmaxf(sumsq[c0 + j] * inv - mu * mu, 0.f);
       const float rs = rsqrtf(var + eps);
       float v = (f[j] - mu) * rs * gamma[c0 + j] + beta[c0 + j];
       o[j] = relu ? fmaxf(v, 0.f) : v;
@@ -819,55 +835,75 @@ extern "C" int tepd_cast_f32_bf16(const void* in, void* out, long long n, void* 
   return (int)cudaGetLastError();
 }
 
-// ---- BatchNorm NHWC.  ws: fp32 [2, C] scratch, zeroed by the caller (sum / sumsq, or sum(dy) / sum(dy*xhat) which the
-// backward ALSO adds into dbeta / dgamma: the caller points ws at zero-filled temporaries and accumulates them itself).
+// ---- BatchNorm NHWC.  ws: fp32 [2, C] scratch, zeroed by the caller (sum / centred sum of squares, or sum(dy) / sum(dy*xhat)
+// which the backward ALSO adds into dbeta / dgamma: the caller points ws at zero-filled temporaries and accumulates them itself).
+namespace {
+dim3 bn_reduce_grid(int rows, int C) { return dim3((C + 255) / 256, (rows + 127) / 128); }
+template <int MODE>
+cudaError_t bn_reduce(const void* a, const void* x, const void* mean, const void* rstd, void* ws, int rows, int C, float count,
+                      void* stream) {
+  float* w = (float*)ws;
+  return tepd::launch(bn_reduce2_kernel<MODE>, bn_reduce_grid(rows, C), dim3(256), 0, CS(stream), (const bf16*)a, (const bf16*)x,
+                      (const float*)mean, (const float*)rstd, w, w + C, rows, C, 128, count);
+}
+template <bool CENTRED>
+cudaError_t bn_fwd_apply(const void* x, const void* ws, const void* gamma, const void* beta, void* y, void* mean, void* rstd, int rows,
+                         int C, float eps, int relu, float count, void* stream) {
+  const float* w = (const float*)ws;
+  return tepd::launch(bn_fwd_apply_kernel<CENTRED>, dim3(grid_for((size_t)rows * C / 8, 256)), dim3(256), 0, CS(stream), (const bf16*)x,
+                      w, w + C, (const float*)gamma, (const float*)beta, (bf16*)y, (float*)mean, (float*)rstd, rows, C, eps, relu, count);
+}
+}  // namespace
+
 extern "C" int tepd_bn_fwd_nhwc(const void* x, const void* gamma, const void* beta, void* y, void* mean, void* rstd, void* ws,
                                 int rows, int C, float eps, int relu, void* stream) {
   if (C % 8) return -2;
-  const int rpb = 128;
-  dim3 grid((C + 255) / 256, (rows + rpb - 1) / rpb);
-  float* w = (float*)ws;
-  cudaError_t e = tepd::launch(bn_reduce2_kernel<0>, grid, dim3(256), 0, CS(stream), (const bf16*)x, (const bf16*)nullptr,
-                               (const float*)nullptr, (const float*)nullptr, w, w + C, rows, C, rpb);
+  cudaError_t e = bn_reduce<2>(x, nullptr, nullptr, nullptr, ws, rows, C, (float)rows, stream);
+  if (e == cudaSuccess) e = bn_reduce<3>(x, nullptr, nullptr, nullptr, ws, rows, C, (float)rows, stream);
   if (e != cudaSuccess) return (int)e;
-  return (int)tepd::launch(bn_fwd_apply_kernel, dim3(grid_for((size_t)rows * C / 8, 256)), dim3(256), 0, CS(stream), (const bf16*)x,
-                           (const float*)w, (const float*)(w + C), (const float*)gamma, (const float*)beta, (bf16*)y, (float*)mean,
-                           (float*)rstd, rows, C, eps, relu, (float)rows);
+  return (int)bn_fwd_apply<true>(x, ws, gamma, beta, y, mean, rstd, rows, C, eps, relu, (float)rows, stream);
 }
 extern "C" int tepd_bn_bwd_nhwc(const void* dy, const void* x, const void* gamma, const void* mean, const void* rstd, void* dx,
                                 void* ws, int rows, int C, void* stream) {
   if (C % 8) return -2;
-  const int rpb = 128;
-  dim3 grid((C + 255) / 256, (rows + rpb - 1) / rpb);
-  float* w = (float*)ws;
-  cudaError_t e = tepd::launch(bn_reduce2_kernel<1>, grid, dim3(256), 0, CS(stream), (const bf16*)dy, (const bf16*)x,
-                               (const float*)mean, (const float*)rstd, w, w + C, rows, C, rpb);
+  const cudaError_t e = bn_reduce<1>(dy, x, mean, rstd, ws, rows, C, (float)rows, stream);
   if (e != cudaSuccess) return (int)e;
+  const float* w = (const float*)ws;
   return (int)tepd::launch(bn_bwd_apply_kernel, dim3(grid_for((size_t)rows * C / 8, 256)), dim3(256), 0, CS(stream), (const bf16*)dy,
-                           (const bf16*)x, (const float*)gamma, (const float*)mean, (const float*)rstd, (const float*)w,
-                           (const float*)(w + C), (bf16*)dx, rows, C, (float)rows);
+                           (const bf16*)x, (const float*)gamma, (const float*)mean, (const float*)rstd, w, w + C, (bf16*)dx, rows, C,
+                           (float)rows);
 }
 // Split-phase BatchNorm for a batch that is split over devices (synchronised BatchNorm): the per-channel sums of the local
-// shard are produced by `tepd_bn_reduce_nhwc`, completed across the devices by an all-reduce of the 2 x C words, and consumed
-// by the apply halves with the GLOBAL row count.  mode 0: ws = [sum(x), sum(x^2)]; mode 1: ws = [sum(dy), sum(dy * xhat)].
+// shard are produced by the reduce entry points, completed across the devices by an all-reduce, and consumed by the apply
+// halves with the GLOBAL row count.
+//   forward : tepd_bn_reduce_nhwc mode 2 (ws[0] = sum(x)), all-reduce ws[0], tepd_bn_centred_sq_nhwc (ws[1] = sum((x - mean)^2)
+//             with the global mean), all-reduce ws[1], tepd_bn_fwd_apply_centred_nhwc.  Every shard shifts by the same mean,
+//             so the all-reduced ws[1] is the centred second moment of the whole batch.
+//   backward: tepd_bn_reduce_nhwc mode 1 (ws = [sum(dy), sum(dy * xhat)]), all-reduce ws, tepd_bn_bwd_apply_nhwc.
+// mode 0 (ws = [sum(x), sum(x^2)]) with tepd_bn_fwd_apply_nhwc is the one-pass forward, which cancels when |mean| >> std.
 extern "C" int tepd_bn_reduce_nhwc(const void* a, const void* x, const void* mean, const void* rstd, void* ws, int rows, int C, int mode,
                                    void* stream) {
   if (C % 8) return -2;
-  const int rpb = 128;
-  dim3 grid((C + 255) / 256, (rows + rpb - 1) / rpb);
-  float* w = (float*)ws;
-  if (mode == 0)
-    return (int)tepd::launch(bn_reduce2_kernel<0>, grid, dim3(256), 0, CS(stream), (const bf16*)a, (const bf16*)nullptr,
-                             (const float*)nullptr, (const float*)nullptr, w, w + C, rows, C, rpb);
-  return (int)tepd::launch(bn_reduce2_kernel<1>, grid, dim3(256), 0, CS(stream), (const bf16*)a, (const bf16*)x, (const float*)mean,
-                           (const float*)rstd, w, w + C, rows, C, rpb);
+  if (mode == 0) return (int)bn_reduce<0>(a, nullptr, nullptr, nullptr, ws, rows, C, 0.f, stream);
+  if (mode == 1) return (int)bn_reduce<1>(a, x, mean, rstd, ws, rows, C, 0.f, stream);
+  if (mode == 2) return (int)bn_reduce<2>(a, nullptr, nullptr, nullptr, ws, rows, C, 0.f, stream);
+  return -3;
+}
+// ws[1] += sum over this shard's rows of (x - ws[0] / count)^2; ws[0] must hold sum(x) over the global batch of `count` rows
+extern "C" int tepd_bn_centred_sq_nhwc(const void* x, void* ws, int rows, int C, float count, void* stream) {
+  if (C % 8) return -2;
+  return (int)bn_reduce<3>(x, nullptr, nullptr, nullptr, ws, rows, C, count, stream);
 }
 extern "C" int tepd_bn_fwd_apply_nhwc(const void* x, const void* ws, const void* gamma, const void* beta, void* y, void* mean, void* rstd,
                                       int rows, int C, float eps, int relu, float count, void* stream) {
   if (C % 8) return -2;
-  const float* w = (const float*)ws;
-  return (int)tepd::launch(bn_fwd_apply_kernel, dim3(grid_for((size_t)rows * C / 8, 256)), dim3(256), 0, CS(stream), (const bf16*)x, w,
-                           w + C, (const float*)gamma, (const float*)beta, (bf16*)y, (float*)mean, (float*)rstd, rows, C, eps, relu, count);
+  return (int)bn_fwd_apply<false>(x, ws, gamma, beta, y, mean, rstd, rows, C, eps, relu, count, stream);
+}
+// ws = [sum(x), sum((x - mean)^2)] over the global batch of `count` rows
+extern "C" int tepd_bn_fwd_apply_centred_nhwc(const void* x, const void* ws, const void* gamma, const void* beta, void* y, void* mean,
+                                              void* rstd, int rows, int C, float eps, int relu, float count, void* stream) {
+  if (C % 8) return -2;
+  return (int)bn_fwd_apply<true>(x, ws, gamma, beta, y, mean, rstd, rows, C, eps, relu, count, stream);
 }
 extern "C" int tepd_bn_bwd_apply_nhwc(const void* dy, const void* x, const void* gamma, const void* mean, const void* rstd, const void* ws,
                                       void* dx, int rows, int C, float count, void* stream) {

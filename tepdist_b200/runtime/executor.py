@@ -1031,7 +1031,8 @@ class Executor:
         else:
             dy, xx, gm = ins
         if ops.bn_native_ok(xx) and os.environ.get("TEPDIST_BN_SYNC", "native") == "native":
-            # native split phases: local sums kernel -> all-reduce of 2 x C floats -> apply kernel with the global count
+            # native split phases: local sums kernel -> all-reduce -> apply kernel with the global count (forward: sum(x), then
+            # the centred sum of squares around the global mean, one all-reduce of C floats each; backward: one of 2 x C)
             shards = 1
             for _, num in levels:
                 shards *= num

@@ -667,8 +667,9 @@ def grad_tol(name):
     return GRAD_TOL[re.sub(r"^model/(h0/)?", "", name)]
 
 
-def step_checks(gpu, cpu, feeds_gpu, feeds_cpu, label):
-    """One GPU step with the CPU oracle run from the same fp32 master / m / v, then the gradient table and the update."""
+def step_checks(gpu, cpu, feeds_gpu, feeds_cpu, label, tol=grad_tol):
+    """One GPU step with the CPU oracle run from the same fp32 master / m / v, then the gradient table (bound per parameter
+    name from `tol`) and the update."""
     gs, cs = gpu.store, cpu.store
     assert gs.total == cs.total and gs.order == cs.order
     for name in ("master", "m", "v"):
@@ -689,9 +690,9 @@ def step_checks(gpu, cpu, feeds_gpu, feeds_cpu, label):
         g, r = gs.grad_view(pid).double().cpu(), cs.grad_view(pid).double()
         rel = float((g - r).norm() / r.norm().clamp_min(1e-30))
         worst[name] = rel
-        print(f"  {name:<32} {float(r.norm()):>10.3e} {rel:>9.2e} {grad_tol(name):>8.1e}")
+        print(f"  {name:<32} {float(r.norm()):>10.3e} {rel:>9.2e} {tol(name):>8.1e}")
     for name, rel in worst.items():
-        assert rel <= grad_tol(name), f"{label}: gradient of {name} off by {rel:.3e} relative (bound {grad_tol(name)})"
+        assert rel <= tol(name), f"{label}: gradient of {name} off by {rel:.3e} relative (bound {tol(name)})"
     # the update: fp64 AdamW of the GPU's own gradient, pre-step master / m / v and this step's hyper
     o = gpu.opt
     p_ref, m_ref, v_ref, (tp, tm, tv) = adamw_ref(pre["master"], gs.grad, pre["m"], pre["v"], gpu.hyper[:4], gs.n_decay,
