@@ -12,12 +12,6 @@ if which == "gemm":
     W = torch.randn(N, K, device="cuda", dtype=torch.bfloat16)
     for _ in range(12):
         ops.gemm(A, W, block_n=256)
-elif which == "gemm2":
-    M, N, K = 4096, 4096, 1024
-    A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
-    W = torch.randn(N, K, device="cuda", dtype=torch.bfloat16)
-    for _ in range(12):
-        ops.gemm2(A, W)
 elif which == "attn":
     qkv = torch.randn(4, 1024, 16, 3, 64, device="cuda", dtype=torch.bfloat16)
     q, k, v = qkv[:, :, :, 0], qkv[:, :, :, 1], qkv[:, :, :, 2]
@@ -47,7 +41,7 @@ elif which == "ln":
         y, mean, rstd = ops.layernorm_fwd(x, gmm, bta)
         ops.layernorm_bwd(torch.randn_like(y), x, gmm, mean, rstd, dg, db, dres=x)
 torch.cuda.synchronize()
-if which == "gemm2_final":      # the three hot instantiations of the 2-CTA kernel as the GPT-2 step uses them
+if which == "gemm_step":        # the GEMM kernel's three operand layouts as the GPT-2 step uses them
     M, N, K = 4096, 4096, 1024
     A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
     W = torch.randn(N, K, device="cuda", dtype=torch.bfloat16)

@@ -9,11 +9,10 @@
 # What each tool can and cannot tell us here:
 #   memcheck  : out-of-bounds / misaligned global + shared accesses of the generic proxy (epilogues, im2col, LN, ...).
 #   racecheck : SHARED-memory hazards only (P / dS tiles, LN-bwd accumulators, colsum scratch).  It does NOT see the
-#               global-memory flag protocols (symm_barrier, stream-K partial-tile flags).
+#               global-memory flag protocol of symm_barrier.
 #   synccheck : named-barrier / __syncwarp misuse (bar.sync 1,128 in the epilogues, softmax max exchange).
-#   initcheck : reads of never-written global memory (stream-K workspace, dQ accumulator).
+#   initcheck : reads of never-written global memory (dQ accumulator).
 # Unknown until run: how much of the async proxy (TMA loads, wgmma operand reads) the sanitizer models on sm_90a.
-# `gemm2` is left out by default: its check interleaves numerics with long timing loops.
 set -u
 tool="${1:-memcheck}"
 shift || true

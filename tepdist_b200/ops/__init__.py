@@ -148,6 +148,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     ``accumulate`` adds into an fp32 ``out`` (gradient accumulation / split-K reduction target).
     ``act="gelu"`` with ``out2``: ``out`` receives the pre-activation, ``out2`` the activated value (one pass).
     ``act="gelu_bwd"`` with ``aux`` (pre-activation): the result is multiplied by GELU'(aux) in the epilogue.
+    ``split_k``: 0 = automatic, 1 = one unit per output tile, s > 1 = split-K over s units, -1 = stream-K.  Split-K and
+    stream-K units add their partials into ``out``, so they need ``accumulate`` with an fp32 ``out``.
     """
     assert a.dim() == b.dim() and a.dim() in (2, 3)
     batched = a.dim() == 3
@@ -164,6 +166,9 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
         out = torch.empty(shape, dtype=out_dtype, device=a.device)
         assert not accumulate
     out3 = out.unsqueeze(0) if out.dim() == 2 else out
+    if split_k not in (0, 1) and not (accumulate and out.dtype == torch.float32):
+        raise ValueError(f"gemm: split_k={split_k} adds partial tiles into out, which needs accumulate=True and an fp32 out; "
+                         f"got accumulate={accumulate}, out {out.dtype}")
 
     odd = a.is_cuda and (N % 8 != 0 or (a_mn and M % 8 != 0) or (K % 8 != 0 and not (a_mn and b_mn))
                          or a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16)
@@ -202,13 +207,6 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
         if t is not None and (t.dtype != torch.bfloat16 or t.shape != out.shape or t.stride() != out.stride()):
             raise ValueError(f"gemm: {name} must be bf16 with out's shape {tuple(out.shape)} and strides {out.stride()}; "
                              f"got {t.dtype} {tuple(t.shape)} strides {t.stride()}")
-    if STREAM_K_FWD and split_k == 0 and block_n == 0 and not batched and not accumulate and K >= 512:
-        # wave quantisation check for the persistent 128x256 schedule: below ~93 % SM occupancy the stream-K schedule
-        # (equal k-block ranges per SM + workspace fix-up of split tiles) wins over both tile-parallel kernels
-        tiles = ((M + 127) // 128) * ((N + 255) // 256)
-        waves = -(-tiles // _sms())
-        if tiles / (waves * _sms()) < 0.93:
-            split_k = -1
     if bias is not None:
         assert bias.dtype in (torch.float32, torch.bfloat16) and bias.is_contiguous()
     res3 = None
@@ -220,7 +218,7 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
         if accumulate and out.dtype == torch.float32:
             tiles = ((M + 127) // 128) * ((N + 255) // 256) * batch
             kb = (K + 63) // 64
-            if STREAM_K and tiles >= _sms():
+            if tiles >= _sms():
                 split_k = -1    # stream-K: every SM gets the same number of k-blocks (fp32 red.add flush per tile) once there
                                 # is at least one full wave of tiles; below that plain split-K
             else:
@@ -240,43 +238,11 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     return out
 
 
-STREAM_K_FWD = os.environ.get("TEPDIST_STREAM_K_FWD", "0") == "1"   # stream-K + fix-up for bf16-output GEMMs (opt-in)
-STREAM_K = os.environ.get("TEPDIST_STREAM_K", "1") == "1"  # stream-K scheduling for fp32-accumulate GEMMs (weight gradients)
-
-
 def wgrad_prefers_store(n_out: int, k_in: int) -> bool:
     """Weight gradient [n_out, k_in]: plain-store GEMM when its 128x256 tiles fill at least half of the SMs; smaller outputs
     are better off split over K with fp32 red.add into a zero-filled slot."""
     tiles = ((n_out + 127) // 128) * ((k_in + 255) // 256)
     return n_out >= 256 and k_in >= 256 and n_out % 8 == 0 and k_in % 8 == 0 and tiles >= _sms() // 2
-
-
-def _gemm2_stream_k(M: int, N: int, K: int, fp32_out: bool) -> bool:
-    """Stream-K only for very large plain-store outputs (the lm_head weight gradient); on the transformer shapes the fix-up
-    of split tiles (fp32 partial tiles through L2) costs more than the idle tail wave it removes."""
-    if not STREAM_K or not fp32_out:
-        return False
-    tiles = ((M + 127) // 128) * ((N + 255) // 256)
-    return tiles >= 8 * _sms()
-
-
-def gemm2(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = False, bias: Optional[torch.Tensor] = None,
-          residual: Optional[torch.Tensor] = None, act: Optional[str] = None, out: Optional[torch.Tensor] = None,
-          out2: Optional[torch.Tensor] = None, aux: Optional[torch.Tensor] = None, alpha: float = 1.0,
-          out_dtype: torch.dtype = torch.bfloat16, stream_k: Optional[bool] = None) -> torch.Tensor:
-    """Large-tile GEMM (128x256 output tile per CTA) with an explicit schedule choice: a [M,K] (or [K,M] with a_mn),
-    b [N,K] (or [K,N] with b_mn); bf16 output with the fused epilogues or fp32 plain stores.  stream_k: None = decide
-    from the output size, True = stream-K with fix-up of split tiles, False = one tile per CTA at a time."""
-    M, K = (a.shape[1], a.shape[0]) if a_mn else a.shape
-    N = b.shape[1] if b_mn else b.shape[0]
-    if out is None:
-        out = torch.empty(M, N, dtype=out_dtype, device=a.device)
-    assert a.is_cuda and a.dtype == torch.bfloat16 and a.stride(1) == 1 and b.stride(1) == 1 and out.stride(1) == 1
-    assert out.dtype in (torch.bfloat16, torch.float32)
-    if stream_k is None:
-        stream_k = _gemm2_stream_k(M, N, K, out.dtype == torch.float32)
-    return gemm(a, b, a_mn=a_mn, b_mn=b_mn, bias=bias, residual=residual, act=act, out=out, alpha=alpha,
-                split_k=-1 if stream_k else 1, block_n=256, out2=out2, aux=aux)
 
 
 def einsum(eq: str, a: torch.Tensor, b: torch.Tensor, _force: bool = False) -> torch.Tensor:

@@ -16,9 +16,6 @@
 #include "sm90_ptx.cuh"
 #include "launch.cuh"
 #include <stdio.h>
-#include <map>
-#include <mutex>
-#include <utility>
 
 using namespace sm90;
 
@@ -46,8 +43,6 @@ struct GemmParams {
   int bias_bf16;
   void* D2;        // act 1: when set, D receives the pre-activation and D2 the activated value (saved for backward)
   const void* aux; // act 2: bf16 [b, M, N] pre-activation
-  float* sk_ws;        // stream-K fix-up workspace: [CTA][BLOCK_M][BLOCK_N] fp32 partial tiles
-  unsigned* sk_cnt;    // per CTA: 1 = its partial tile is complete (reset to 0 by the consumer)
   const float* row_scale;  // fp8: per-row activation scale [b, M] (nullptr: none); multiplied with w_scale[b]
   const float* w_scale;
   long long bias_stride;   // bias batch stride (elements): 0 = one bias for every batch
@@ -98,9 +93,6 @@ __device__ __forceinline__ void next_work(const GemmParams& p, int& cursor, int 
   }
 }
 
-// kept out of line: a trap inlined into the kernel stops ptxas from giving the consumers the registers of setmaxnreg.inc
-__device__ __noinline__ void trap_stream_k_timeout() { __trap(); }
-
 __device__ __forceinline__ float gelu_tanh_grad(float x) {
   const float k0 = 0.7978845608028654f, k1 = 0.044715f;
   float t;
@@ -116,9 +108,9 @@ __device__ __forceinline__ float gelu_tanh(float x) {
 }
 
 // Epilogue kinds, fixed at compile time.  EPI_DIRECT stores straight from the accumulator fragments and reads its options
-// (bias, GELU, GELU', residual, fp32 store, red.add, stream-K partials) at run time.  The other kinds write their output
-// through a shared-memory staging buffer (one 64 x BLOCK_N bf16 buffer per consumer warpgroup, in the TMA store box layout)
-// and TMA stores; their inputs are in shared memory before the epilogue starts: the bias (zeros when there is none) is
+// (bias, GELU, GELU', residual, fp32 store, red.add) at run time.  The other kinds write their output through a
+// shared-memory staging buffer (one 64 x BLOCK_N bf16 buffer per consumer warpgroup, in the TMA store box layout) and TMA
+// stores; their inputs are in shared memory before the epilogue starts: the bias (zeros when there is none) is
 // copied there at the start of the tile, the residual / GELU' aux tile is TMA-loaded into the staging buffer itself.  The
 // fp32 kinds fill the same buffer with half the tile's columns at a time (64 x BLOCK_N / 2 fp32) and store it in two rounds.
 enum Epi : int {
@@ -155,7 +147,7 @@ __device__ __forceinline__ float2 ldg_bf16x2(const void* p) {
   return __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(p)));
 }
 
-// named barrier of one consumer warpgroup (ids 2, 3; id 1 spans both consumer warpgroups)
+// named barrier of one consumer warpgroup (ids 2, 3)
 __device__ __forceinline__ void wg_bar_sync(int wg) {
   if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
   else         asm volatile("bar.sync 3, 128;" ::: "memory");
@@ -311,7 +303,6 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
     int cursor, cend;
     work_range(p, cursor, cend);
     while (cursor < cend) {
-      const int tile = cursor;
       Work w;
       next_work(p, cursor, cend, w);
       const int m_blk = w.m_blk, n_blk = w.n_blk;
@@ -440,71 +431,19 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
         }
         continue;
       }
-      // stream-K units that cover only part of a tile's K range (outputs with a real epilogue): a unit that starts
-      // mid-tile (always a CTA's FIRST unit) stores its fp32 partial tile into workspace slot [blockIdx.x] and raises
-      // flag[blockIdx.x]; the unit that holds k-block 0 (always a CTA's LAST unit) is the finisher: it waits for the
-      // flags of the CTAs that follow it inside the tile, adds their partials to its own accumulator and runs the real
-      // epilogue.  Producers never wait and finish their part first, so the wait is short and cannot deadlock.
-      const bool sk_part = p.stream_k > 0 && !p.accumulate && !(w.kb0 == 0 && w.kb1 == p.k_blocks);
-      const bool sk_store = sk_part && w.kb0 > 0;
-      const bool sk_finish = sk_part && w.kb0 == 0;
-      int partner_end = 0;   // finisher: partners are CTAs blockIdx.x+1 .. partner_end-1
-      if (sk_finish) {
-        const int tile_end = tile + p.k_blocks;   // (cursor before next_work == first iteration of the tile)
-        partner_end = blockIdx.x + 1;
-        while (partner_end < (int)gridDim.x && partner_end * p.stream_k < tile_end) ++partner_end;
-        if (threadIdx.x == 0) {
-          for (int j = blockIdx.x + 1; j < partner_end; ++j) {
-            unsigned f;
-            const long long t0 = clock64();
-            do {
-              asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(f) : "l"(p.sk_cnt + j) : "memory");
-              if (f == 0u && clock64() - t0 > 4000000000LL) trap_stream_k_timeout();   // a partner never arrived: fail loudly
-            } while (f == 0u);
-          }
-        }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-      }
       if (has_k) {
         const float* scale_rows = p.row_scale ? p.row_scale + (long long)b * p.M : nullptr;
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
-          const int row_in_tile = row_base + hr * 8;
-          const int row = m_blk * BLOCK_M + row_in_tile;
+          const int row = m_blk * BLOCK_M + row_base + hr * 8;
           if (row >= p.M) continue;
           float alpha = p.alpha;
           if (scale_rows) alpha *= scale_rows[row] * p.w_scale[b];
 #pragma unroll
           for (int j = 0; j < BLOCK_N / 8; ++j) {
-            const int cit = j * 8 + 2 * q;   // column inside the tile
-            const int col = n_blk * BLOCK_N + cit;
+            const int col = n_blk * BLOCK_N + j * 8 + 2 * q;
             if (col >= p.N) continue;
-            float v0 = acc[4 * j + 2 * hr] * alpha, v1 = acc[4 * j + 2 * hr + 1] * alpha;
-            float* wp = p.sk_ws + ((long long)blockIdx.x * BLOCK_M + row_in_tile) * 256 + cit;
-            if (sk_store) {
-              *reinterpret_cast<float2*>(wp) = make_float2(v0, v1);
-              continue;
-            }
-            if (sk_finish) {
-              for (int jj = blockIdx.x + 1; jj < partner_end; ++jj) {
-                float2 t;
-                asm volatile("ld.global.cg.v2.f32 {%0,%1}, [%2];" : "=f"(t.x), "=f"(t.y)
-                             : "l"(p.sk_ws + ((long long)jj * BLOCK_M + row_in_tile) * 256 + cit));
-                v0 += t.x; v1 += t.y;
-              }
-            }
-            epilogue_pair(v0, v1, p, row, col, b, add_bias, add_res);
-          }
-        }
-      }
-      if (sk_part) {
-        if (sk_store) __threadfence();
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (threadIdx.x == 0) {
-          if (sk_store) {
-            asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p.sk_cnt + blockIdx.x), "r"(1u) : "memory");
-          } else {
-            for (int j = blockIdx.x + 1; j < partner_end; ++j) p.sk_cnt[j] = 0u;   // consumed: clean for the next launch
+            epilogue_pair(acc[4 * j + 2 * hr] * alpha, acc[4 * j + 2 * hr + 1] * alpha, p, row, col, b, add_bias, add_res);
           }
         }
       }
@@ -608,51 +547,16 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
   p.m_blocks = (M + BLOCK_M - 1) / BLOCK_M;
   p.n_blocks = (N + block_n - 1) / block_n;
   p.k_blocks = (K + BLOCK_K - 1) / BLOCK_K;
-  p.stream_k = 0; p.sk_ws = nullptr; p.sk_cnt = nullptr;
+  p.stream_k = 0;
   if (num_sms <= 0) num_sms = tepd::num_sms();
   if (split_k < 0) {  // stream-K requested: equal k-block ranges per SM
+    // a unit that ends mid-tile adds its partial into the output, so only an accumulating fp32 output can take it
+    if (!(out_fp32 && accumulate)) return -4;
     const long long iters = (long long)p.m_blocks * p.n_blocks * batch * p.k_blocks;
     long long per = (iters + num_sms - 1) / num_sms;
     if (per < 4) per = 4;   // do not shred tiny problems into sub-4-k-block units
     p.stream_k = (int)per;
     split_k = 1;
-    if (!(out_fp32 && accumulate)) {
-      // outputs with a real epilogue: partial tiles travel through a per-device fp32 workspace (one slot per CTA);
-      // allocated once; flags are reset by their consumer.  GEMMs of one device must not run concurrently on two
-      // streams in this mode.
-      constexpr int kSlots = 160;
-      // pool of workspaces per device, all allocated at the first call (the executor's eager warm-up step, i.e. outside
-      // CUDA-graph capture); every stream is bound to one of them in order of first appearance (binding allocates nothing,
-      // so it may happen during capture), so stream-K GEMMs on up to kPool concurrent streams never share partial tiles
-      constexpr int kPool = 4;
-      struct SkWs { float* ws; unsigned* cnt; };
-      struct DevPool { bool ready = false; SkWs w[kPool]; std::map<void*, int> bound; int next = 0; };
-      static DevPool pools[16];
-      static std::mutex pool_mu;
-      int dev = 0;
-      cudaGetDevice(&dev);
-      if (num_sms + 1 > kSlots || dev >= 16) return -6;
-      SkWs w;
-      {
-        std::lock_guard<std::mutex> lk(pool_mu);
-        DevPool& dp = pools[dev];
-        if (!dp.ready) {
-          const size_t bytes = (size_t)kSlots * BLOCK_M * 256 * sizeof(float);
-          for (int i = 0; i < kPool; ++i) {
-            if (cudaMalloc(&dp.w[i].ws, bytes) != cudaSuccess) return -7;
-            if (cudaMalloc(&dp.w[i].cnt, kSlots * sizeof(unsigned)) != cudaSuccess) return -7;
-            cudaMemset(dp.w[i].ws, 0, bytes);
-            cudaMemset(dp.w[i].cnt, 0, kSlots * sizeof(unsigned));
-          }
-          cudaDeviceSynchronize();
-          dp.ready = true;
-        }
-        auto it = dp.bound.find(stream);
-        if (it == dp.bound.end()) it = dp.bound.emplace(stream, dp.next++ % kPool).first;
-        w = dp.w[it->second];
-      }
-      p.sk_ws = w.ws; p.sk_cnt = w.cnt;
-    }
   }
   if (split_k < 1) split_k = 1;
   if (split_k > p.k_blocks) split_k = p.k_blocks;
@@ -682,12 +586,11 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
   // flags and the operand layout: plain for every layout, bias / bias + residual / dual GELU for the forward layout
   // (A and B K-major), GELU' for the data-gradient layout (B MN-major).  fp32 outputs of the weight-gradient layout (A and B
   // MN-major) without bias, residual or activation go through shared memory too: plain stores, or TMA reduce-adds for
-  // accumulating outputs (split-K, stream-K, gradient accumulation); a stream-K fix-up of a plain store stays direct.
-  // Everything else stores from the fragments.
+  // accumulating outputs (split-K, stream-K, gradient accumulation).  Everything else stores from the fragments.
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   const bool fwd = !a_mn && !b_mn, dgrad = !a_mn && b_mn, wgrad = a_mn && b_mn;
   int epi = EPI_DIRECT;
-  if (!out_fp32 && p.stream_k == 0 && ldd % 8 == 0 && (batch == 1 || stride_d % 8 == 0) && al16(D)) {
+  if (!out_fp32 && ldd % 8 == 0 && (batch == 1 || stride_d % 8 == 0) && al16(D)) {
     const bool res_ok = residual != nullptr && al16(residual) && ld_res % 8 == 0 && (batch == 1 || stride_res % 8 == 0);
     if (act == 0 && !bias && !residual) epi = EPI_PLAIN;
     else if (act == 0 && !residual && fwd) epi = EPI_BIAS;
@@ -695,8 +598,7 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
     else if (act == 1 && D2 && al16(D2) && !residual && fwd) epi = EPI_GELU_DUAL;
     else if (act == 2 && al16(aux) && !bias && !residual && dgrad) epi = EPI_GELU_BWD;
   }
-  if (out_fp32 && wgrad && act == 0 && !bias && !residual && (accumulate || p.stream_k == 0) && ldd % 4 == 0 &&
-      (batch == 1 || stride_d % 4 == 0) && al16(D))
+  if (out_fp32 && wgrad && act == 0 && !bias && !residual && ldd % 4 == 0 && (batch == 1 || stride_d % 4 == 0) && al16(D))
     epi = accumulate ? EPI_F32_ADD : EPI_F32;
   Maps m;
   m.a = ta; m.b = tb;
@@ -752,7 +654,7 @@ extern "C" int tepd_gemm_fp8(const void* A, const void* B, void* D, const void* 
   GemmParams p;
   p.M = M; p.N = N; p.K = K; p.batch = batch;
   p.m_blocks = (M + BLOCK_M - 1) / BLOCK_M; p.n_blocks = (N + BN - 1) / BN; p.k_blocks = (K + 127) / 128;
-  p.split_k = 1; p.stream_k = 0; p.sk_ws = nullptr; p.sk_cnt = nullptr;
+  p.split_k = 1; p.stream_k = 0;
   p.ldd = N; p.stride_d = (long long)M * N; p.ld_res = 0; p.stride_res = 0;
   p.D = D; p.bias = bias; p.residual = nullptr; p.alpha = 1.0f;
   p.out_fp32 = 0; p.accumulate = 0; p.act = act == 1 ? 1 : 0; p.bias_bf16 = 0; p.D2 = nullptr; p.aux = nullptr;

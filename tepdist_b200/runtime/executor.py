@@ -35,8 +35,6 @@ TP_FUSED_IMPL = None
 # GPT-MoE: dispatch / combine einsums whose mask comes from moe_dispatch_mask run as route-table row gathers (ops.moe_*), not as
 # dense [G,S,E*C] x [G,S,M] GEMMs; TEPDIST_MOE_SPARSE=0 keeps the dense einsums (the comparator)
 MOE_SPARSE = os.environ.get("TEPDIST_MOE_SPARSE", "1") == "1"
-# weight gradients with a single producer are written with plain stores instead of fp32 atomics into a zero-filled slot
-WGRAD_PLAIN_STORE = os.environ.get("TEPDIST_WGRAD_STORE", "1") == "1"
 
 _TORCH_DTYPE = {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32, "i32": torch.int32,
                 "i64": torch.int64, "bool": torch.bool}
@@ -1209,7 +1207,7 @@ class Executor:
         contiguous ranges of the flat gradient buffer."""
         self._store_init: set = set()
         self._zero_ranges: Optional[List[Tuple[int, int]]] = None
-        if not WGRAD_PLAIN_STORE or self.grad_accumulate or not self.store.master.is_cuda:
+        if self.grad_accumulate or not self.store.master.is_cuda:
             return
         st = self.store
         self_init_params = set()

@@ -111,24 +111,6 @@ def check_gemm_epilogues():
     acc = torch.zeros(M, N, device="cuda", dtype=torch.float32)
     ops.gemm(A, W, bias=bs, out=acc, accumulate=True, split_k=-1)
     out["streamk_bias"] = _rel_err(acc, A.float() @ W.float().t() + bs)
-    # stream-K with workspace fix-up for outputs that have a real epilogue (bf16 / fp32 stores, bias, GELU, residual);
-    # run every case twice: the second launch only passes if the finisher left the workspace clean
-    for (Ms, Ns, Ks) in [(4096, 1024, 1024), (4096, 3072, 1024), (1000, 520, 2048), (384, 256, 4096)]:
-        As = torch.randn(Ms, Ks, device="cuda", dtype=torch.bfloat16)
-        Ws = torch.randn(Ns, Ks, device="cuda", dtype=torch.bfloat16) * 0.05
-        bss = torch.randn(Ns, device="cuda", dtype=torch.float32)
-        rs = torch.randn(Ms, Ns, device="cuda", dtype=torch.bfloat16)
-        refs = As.float() @ Ws.float().t() + bss
-        for rep in range(2):
-            d = ops.gemm(As, Ws, bias=bss, residual=rs, split_k=-1)
-            out[f"skfix_res_{Ms}x{Ns}x{Ks}_{rep}"] = _rel_err(d, refs + rs.float())
-        d = ops.gemm(As, Ws, bias=bss, act="gelu", split_k=-1)
-        out[f"skfix_gelu_{Ms}x{Ns}x{Ks}"] = _rel_err(d, torch.nn.functional.gelu(refs, approximate="tanh"))
-        d = ops.gemm(As, Ws, out_dtype=torch.float32, split_k=-1)
-        out[f"skfix_fp32_{Ms}x{Ns}x{Ks}"] = _rel_err(d, refs - bss)
-        Wt = Ws.t().contiguous()                        # dgrad layout: B stored [K, N]
-        d = ops.gemm(As, Wt, b_mn=True, split_k=-1)
-        out[f"skfix_bmn_{Ms}x{Ns}x{Ks}"] = _rel_err(d, refs - bss)
     # dual-output GELU (pre-activation + activation in one pass) and fused GELU backward on a dgrad-layout GEMM
     pre, act = torch.empty(M, N, device="cuda", dtype=torch.bfloat16), torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
     ops.gemm(A, W, bias=bias, act="gelu", out=pre, out2=act)
@@ -152,93 +134,6 @@ def check_gemm_epilogues():
     return out
 
 
-def check_gemm2():
-    """ops.gemm2 (128x256 tiles, explicit tile-parallel / stream-K schedule): numerics vs fp32 reference for both B layouts +
-    fused epilogues, then throughput."""
-    from tepdist_b200 import ops
-    out = {}
-    torch.manual_seed(7)
-    for (M, N, K) in [(256, 256, 64), (512, 768, 256), (1024, 1024, 1024), (384, 520, 200)]:
-        A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
-        Bm = torch.randn(K, N, device="cuda", dtype=torch.bfloat16)
-        ref = A.float() @ Bm.float()
-        for b_mn in (False, True):
-            b = Bm if b_mn else Bm.t().contiguous()
-            d = ops.gemm2(A, b, b_mn=b_mn)
-            torch.cuda.synchronize()
-            out[f"{M}x{N}x{K}_bmn{int(b_mn)}"] = _rel_err(d, ref)
-            assert out[f"{M}x{N}x{K}_bmn{int(b_mn)}"] < 1e-2, out
-    M, N, K = 512, 768, 256
-    A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
-    W = torch.randn(N, K, device="cuda", dtype=torch.bfloat16) * 0.05
-    bias = torch.randn(N, device="cuda")
-    res = torch.randn(M, N, device="cuda", dtype=torch.bfloat16)
-    ref = A.float() @ W.float().t() + bias
-    out["bias_res"] = _rel_err(ops.gemm2(A, W, bias=bias, residual=res), ref + res.float())
-    pre, act = torch.empty(M, N, device="cuda", dtype=torch.bfloat16), torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
-    ops.gemm2(A, W, bias=bias, act="gelu", out=pre, out2=act)
-    out["gelu_dual_pre"] = _rel_err(pre, ref)
-    out["gelu_dual_act"] = _rel_err(act, torch.nn.functional.gelu(ref, approximate="tanh"))
-    # stream-K schedule (forced) on shapes whose tiles are split 2 and 3+ ways, every B layout, epilogues, twice in a row
-    for (M, N, K) in [(4096, 1024, 1024), (4096, 3072, 1024), (1000, 520, 2048), (512, 512, 8192), (384, 520, 200)]:
-        A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
-        W = torch.randn(N, K, device="cuda", dtype=torch.bfloat16) * 0.05
-        bias = torch.randn(N, device="cuda")
-        res = torch.randn(M, N, device="cuda", dtype=torch.bfloat16)
-        ref = A.float() @ W.float().t() + bias
-        for rep in range(2):
-            out[f"sk_res_{M}x{N}x{K}_{rep}"] = _rel_err(ops.gemm2(A, W, bias=bias, residual=res, stream_k=True), ref + res.float())
-        out[f"sk_gelu_{M}x{N}x{K}"] = _rel_err(ops.gemm2(A, W, bias=bias, act="gelu", stream_k=True),
-                                               torch.nn.functional.gelu(ref, approximate="tanh"))
-        out[f"sk_bmn_{M}x{N}x{K}"] = _rel_err(ops.gemm2(A, W.t().contiguous(), b_mn=True, stream_k=True), ref - bias)
-    # weight-gradient layout: A [T, N] and B [T, K] both MN-major, fp32 plain stores; tile-parallel and stream-K
-    for (T, N, K) in [(4096, 1024, 1024), (4096, 3072, 1024), (1096, 1000, 520), (8192, 384, 256)]:
-        dY = torch.randn(T, N, device="cuda", dtype=torch.bfloat16)
-        X = torch.randn(T, K, device="cuda", dtype=torch.bfloat16)
-        ref = dY.float().t() @ X.float()
-        for sk in (False, True):
-            d = ops.gemm2(dY, X, a_mn=True, b_mn=True, out_dtype=torch.float32, stream_k=sk)
-            out[f"wgrad_{N}x{K}x{T}_sk{int(sk)}"] = _rel_err(d, ref)
-    for k, v in out.items():
-        assert v < 1e-2, (k, v)
-    perf = {}
-    for (M, N, K, bmn) in [(4096, 3072, 1024, False), (4096, 1024, 1024, False), (4096, 4096, 1024, False), (4096, 1024, 4096, False),
-                           (4096, 1024, 3072, True), (4096, 1024, 4096, True), (4096, 4096, 1024, True), (4096, 50304, 1024, False)]:
-        A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
-        W = torch.randn(K, N, device="cuda", dtype=torch.bfloat16) if bmn else torch.randn(N, K, device="cuda", dtype=torch.bfloat16)
-        tag = f"{M}x{N}x{K}{'_bmn' if bmn else ''}"
-        perf[tag] = {}
-        for nm, sk in (("tile", False), ("streamk", True)):
-            ms = _time_ms(lambda: ops.gemm2(A, W, b_mn=bmn, stream_k=sk))
-            perf[tag][nm] = round(2.0 * M * N * K / ms / 1e9, 1)
-        ms = _time_ms(lambda: torch.matmul(A, W if bmn else W.t()))
-        perf[tag]["cublas"] = round(2.0 * M * N * K / ms / 1e9, 1)
-    T = 4096
-    for (N, K) in [(3072, 1024), (1024, 1024), (4096, 1024), (1024, 4096), (50304, 1024)]:
-        dY = torch.randn(T, N, device="cuda", dtype=torch.bfloat16)
-        X = torch.randn(T, K, device="cuda", dtype=torch.bfloat16)
-        acc = torch.zeros(N, K, device="cuda", dtype=torch.float32)
-        tag = f"wgrad_{N}x{K}"
-        perf[tag] = {}
-        for nm, sk in (("tile", False), ("streamk", True)):
-            ms = _time_ms(lambda: ops.gemm2(dY, X, a_mn=True, b_mn=True, out=acc, stream_k=sk))
-            perf[tag][nm] = round(2.0 * T * N * K / ms / 1e9, 1)
-        ms = _time_ms(lambda: ops.gemm(dY, X, a_mn=True, b_mn=True, out=acc, accumulate=True, split_k=1))
-        perf[tag]["cta1_redadd"] = round(2.0 * T * N * K / ms / 1e9, 1)
-        ms = _time_ms(lambda: torch.matmul(dY.t(), X))
-        perf[tag]["cublas"] = round(2.0 * T * N * K / ms / 1e9, 1)
-    out["perf_tflops"] = perf
-    for (M, N, K) in [(8192, 8192, 8192), (4096, 4096, 1024), (4096, 1024, 4096), (4096, 3072, 1024)]:
-        A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
-        W = torch.randn(N, K, device="cuda", dtype=torch.bfloat16)
-        ms2 = _time_ms(lambda: ops.gemm2(A, W))
-        ms1 = _time_ms(lambda: ops.gemm(A, W, block_n=256))
-        msc = _time_ms(lambda: torch.matmul(A, W.t()))
-        f = 2.0 * M * N * K / 1e9
-        out[f"tflops_{M}x{N}x{K}"] = {"gemm2": f / ms2, "gemm1": f / ms1, "cublas": f / msc}
-    return out
-
-
 def check_gemm_perf():
     from tepdist_b200 import ops
     out = {}
@@ -259,18 +154,14 @@ def check_gemm_perf():
     out["ours_wgrad_4096tok_1024x4096_tflops"] = 2.0 * T * N * K / ms / 1e9
     ms = _time_ms(lambda: torch.matmul(dY.t(), X))
     out["cublas_wgrad_tflops"] = 2.0 * T * N * K / ms / 1e9
-    # stream-K + fix-up vs the tile-parallel schedules (128- and 256-wide tiles) and cuBLAS on the forward and dgrad shapes
+    # the 256-wide tile schedule and cuBLAS on the forward and dgrad shapes
     for (M, N, K, bmn) in [(4096, 3072, 1024, False), (4096, 1024, 1024, False), (4096, 4096, 1024, False), (4096, 1024, 4096, False),
                            (4096, 1024, 3072, True), (4096, 1024, 4096, True), (4096, 4096, 1024, True)]:
         A = torch.randn(M, K, device="cuda", dtype=torch.bfloat16)
         W = torch.randn(K, N, device="cuda", dtype=torch.bfloat16) if bmn else torch.randn(N, K, device="cuda", dtype=torch.bfloat16)
         tag = f"{M}x{N}x{K}{'_bmn' if bmn else ''}"
-        ms = _time_ms(lambda: ops.gemm(A, W, b_mn=bmn, split_k=-1))
-        out[f"streamk_fix_{tag}_tflops"] = 2.0 * M * N * K / ms / 1e9
         ms = _time_ms(lambda: ops.gemm(A, W, b_mn=bmn, block_n=256))
         out[f"cta1_{tag}_tflops"] = 2.0 * M * N * K / ms / 1e9
-        ms = _time_ms(lambda: ops.gemm2(A, W, b_mn=bmn))
-        out[f"cta2_{tag}_tflops"] = 2.0 * M * N * K / ms / 1e9
         ms = _time_ms(lambda: torch.matmul(A, W if bmn else W.t()))
         out[f"cublas_{tag}_tflops"] = 2.0 * M * N * K / ms / 1e9
     # wave-quantisation probe: 33 m-blocks x {4, 16} n-blocks = exact multiples of 132 tiles vs the 32 m-block shapes
@@ -279,8 +170,6 @@ def check_gemm_perf():
         W = torch.randn(N, K, device="cuda", dtype=torch.bfloat16)
         ms = _time_ms(lambda: ops.gemm(A, W, block_n=256))
         out[f"probe_cta1_{M}x{N}x{K}_tflops"] = 2.0 * M * N * K / ms / 1e9
-        ms = _time_ms(lambda: ops.gemm2(A, W))
-        out[f"probe_cta2_{M}x{N}x{K}_tflops"] = 2.0 * M * N * K / ms / 1e9
         ms = _time_ms(lambda: torch.matmul(A, W.t()))
         out[f"probe_cublas_{M}x{N}x{K}_tflops"] = 2.0 * M * N * K / ms / 1e9
     # stream-K vs the data-parallel / split-K schedule on the four GPT-2 345M weight-gradient shapes (4096 tokens)
@@ -290,12 +179,8 @@ def check_gemm_perf():
         acc = torch.zeros(N, K, device="cuda", dtype=torch.float32)
         ms = _time_ms(lambda: ops.gemm(dY, X, a_mn=True, b_mn=True, out=acc, accumulate=False, split_k=1))
         out[f"wgrad_{N}x{K}_plainstore_tflops"] = 2.0 * T * N * K / ms / 1e9
-        for tag, sk in (("streamk", -1), ("dp", 1), ("auto_old", 0)):
-            if tag == "auto_old":
-                ops.STREAM_K, prev = False, ops.STREAM_K
+        for tag, sk in (("streamk", -1), ("dp", 1)):
             ms = _time_ms(lambda: ops.gemm(dY, X, a_mn=True, b_mn=True, out=acc, accumulate=True, split_k=sk))
-            if tag == "auto_old":
-                ops.STREAM_K = prev
             out[f"wgrad_{N}x{K}_{tag}_tflops"] = 2.0 * T * N * K / ms / 1e9
         ms = _time_ms(lambda: torch.matmul(dY.t(), X))
         out[f"wgrad_{N}x{K}_cublas_tflops"] = 2.0 * T * N * K / ms / 1e9
@@ -754,7 +639,6 @@ CHECKS = {
     "moe_routes": check_moe_routes,
     "ew": check_ew,
     "attn_d48": check_attn_d48,
-    "gemm2": check_gemm2,
     "attn_perf": check_attn_perf,
 }
 
