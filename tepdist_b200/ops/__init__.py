@@ -85,7 +85,6 @@ class _Sig:
     tepd_bn_fwd_nhwc = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _i, _vp]
     tepd_bn_bwd_nhwc = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]
     tepd_bn_reduce_nhwc = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]
-    tepd_bn_fwd_apply_nhwc = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _i, _f, _vp]
     tepd_bn_bwd_apply_nhwc = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _vp]
     tepd_bn_centred_sq_nhwc = [_vp, _vp, _i, _i, _f, _vp]
     tepd_bn_fwd_apply_centred_nhwc = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _i, _f, _vp]
@@ -97,7 +96,6 @@ class _Sig:
     tepd_xent_fwd_bwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp]
     tepd_adamw = [_vp, _vp, _vp, _vp, _vp, _ll, _ll, _f, _f, _f, _f, _f, _f, _f, _f, _vp, _vp]
     tepd_sgd = [_vp, _vp, _vp, _ll, _f, _f, _vp]
-    tepd_axpy_f32 = [_vp, _vp, _ll, _f, _vp]
     tepd_cast_f32_bf16 = [_vp, _vp, _ll, _vp]
     tepd_ew_bf16 = [_vp, _vp, _vp, _ll, _i, _vp]
     tepd_moe_gather_scale = [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]
@@ -793,14 +791,6 @@ def sgd_step(p: torch.Tensor, g: torch.Tensor, p_bf16: Optional[torch.Tensor], l
             p_bf16.copy_(p.to(p_bf16.dtype))
         return
     _check(lib().tepd_sgd(p.data_ptr(), g.data_ptr(), _p(p_bf16), p.numel(), lr, grad_scale, _stream()), "sgd")
-    _count()
-
-
-def axpy_f32(acc: torch.Tensor, g: torch.Tensor, a: float = 1.0) -> None:
-    if not acc.is_cuda:
-        acc.add_(g, alpha=a)
-        return
-    _check(lib().tepd_axpy_f32(acc.data_ptr(), g.data_ptr(), acc.numel(), a, _stream()), "axpy_f32")
     _count()
 
 

@@ -242,13 +242,12 @@ __global__ void gelu_bwd_kernel(const uint4* __restrict__ dy, const uint4* __res
 // ------------------------------------------------------------------ BatchNorm (training mode) on NHWC rows
 // x is [rows = N*H*W, C] (channels_last memory).  All passes are column-parallel like colsum:
 //   forward : bn_reduce2 accumulates sum(x) per channel (fp32 atomics over row strips), then the centred second moment
-//             sum((x - mean)^2) with mean = sum(x) / count; bn_fwd_apply<true> turns them into mean / rstd and writes
-//             y = (x - mean) * rstd * gamma + beta (+ ReLU).  The one-pass form E[x^2] - E[x]^2 (MODE 0, apply<false>) loses
-//             all of its digits when |mean| >> std (a channel at mean / std = 300 keeps none of them in fp32), so the
-//             library's own forward no longer uses it; it stays behind the split-phase mode 0 for existing callers.
+//             sum((x - mean)^2) with mean = sum(x) / count; bn_fwd_apply turns them into mean / rstd and writes
+//             y = (x - mean) * rstd * gamma + beta (+ ReLU).  The one-pass form E[x^2] - E[x]^2 is not used: it loses all of
+//             its digits when |mean| >> std (a channel at mean / std = 300 keeps none of them in fp32).
 //   backward: bn_reduce2 with dy accumulates sum(dy) and sum(dy * xhat), bn_bwd_apply writes
 //             dx = gamma * rstd * (dy - mean(dy) - xhat * mean(dy * xhat)).
-// MODE 0: (x, x^2); MODE 1: (dy, dy * xhat) with xhat recomputed from x, mean, rstd; MODE 2: x into out0 only;
+// MODE 1: (dy, dy * xhat) with xhat recomputed from x, mean, rstd; MODE 2: x into out0 only;
 // MODE 3: (x - mu)^2 into out1 only, mu = out0 / count computed exactly as bn_fwd_apply computes it (out0 is only read).
 template <int MODE>
 __global__ void __launch_bounds__(256) bn_reduce2_kernel(const bf16* __restrict__ a, const bf16* __restrict__ x,
@@ -276,10 +275,7 @@ __global__ void __launch_bounds__(256) bn_reduce2_kernel(const bf16* __restrict_
     for (int r = r0 + warp; r < r1; r += 8) {
       float f[8];
       unpack8(__ldg(reinterpret_cast<const uint4*>(a + (size_t)r * C + col0)), f);
-      if (MODE == 0) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { s0[j] += f[j]; s1[j] += f[j] * f[j]; }
-      } else if (MODE == 2) {
+      if (MODE == 2) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) s0[j] += f[j];
       } else if (MODE == 3) {
@@ -306,8 +302,7 @@ __global__ void __launch_bounds__(256) bn_reduce2_kernel(const bf16* __restrict_
   }
 }
 
-// CENTRED: sums = [sum(x), sum((x - mean)^2)], else [sum(x), sum(x^2)] -> mean, rstd (written by block row 0) and y
-template <bool CENTRED>
+// sums = [sum(x), sum((x - mean)^2)] -> mean, rstd (written by block row 0) and y
 __global__ void __launch_bounds__(256) bn_fwd_apply_kernel(const bf16* __restrict__ x, const float* __restrict__ sum,
                                                           const float* __restrict__ sumsq, const float* __restrict__ gamma,
                                                           const float* __restrict__ beta, bf16* __restrict__ y,
@@ -323,7 +318,7 @@ __global__ void __launch_bounds__(256) bn_fwd_apply_kernel(const bf16* __restric
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float mu = sum[c0 + j] * inv;
-      const float var = CENTRED ? sumsq[c0 + j] * inv : fmaxf(sumsq[c0 + j] * inv - mu * mu, 0.f);
+      const float var = sumsq[c0 + j] * inv;
       const float rs = rsqrtf(var + eps);
       float v = (f[j] - mu) * rs * gamma[c0 + j] + beta[c0 + j];
       o[j] = relu ? fmaxf(v, 0.f) : v;
@@ -595,16 +590,6 @@ __global__ void sgd_kernel(float* __restrict__ p, const float* __restrict__ g, b
   }
 }
 
-// acc += g  (gradient accumulation "GA" task on fp32 buffers); cast helper.
-__global__ void axpy_f32_kernel(float* __restrict__ acc, const float* __restrict__ g, size_t n, float a) {
-  const size_t nvec = n >> 2;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nvec; i += (size_t)gridDim.x * blockDim.x) {
-    float4 x = reinterpret_cast<float4*>(acc)[i];
-    float4 y = reinterpret_cast<const float4*>(g)[i];
-    x.x += a * y.x; x.y += a * y.y; x.z += a * y.z; x.w += a * y.w;
-    reinterpret_cast<float4*>(acc)[i] = x;
-  }
-}
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ in, bf16* __restrict__ out, size_t n) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     out[i] = __float2bfloat16(in[i]);
@@ -799,11 +784,6 @@ extern "C" int tepd_sgd(void* p, const void* g, void* p_bf16, long long n, float
   sgd_kernel<<<grid_for(n, 256), 256, 0, CS(stream)>>>((float*)p, (const float*)g, (bf16*)p_bf16, n, lr, gscale);
   return (int)cudaGetLastError();
 }
-extern "C" int tepd_axpy_f32(void* acc, const void* g, long long n, float a, void* stream) {
-  if (n % 4) return -2;
-  axpy_f32_kernel<<<grid_for(n / 4, 256), 256, 0, CS(stream)>>>((float*)acc, (const float*)g, n, a);
-  return (int)cudaGetLastError();
-}
 // out = relu(a) (mode 0) | a * (b > 0) (mode 1: ReLU backward with b = the forward OUTPUT) | a + b (mode 2); n % 8 == 0, 16-byte aligned
 extern "C" int tepd_ew_bf16(const void* a, const void* b, void* out, long long n, int mode, void* stream) {
   if (n % 8 || ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(b)) & 15)) return -2;
@@ -846,11 +826,10 @@ cudaError_t bn_reduce(const void* a, const void* x, const void* mean, const void
   return tepd::launch(bn_reduce2_kernel<MODE>, bn_reduce_grid(rows, C), dim3(256), 0, CS(stream), (const bf16*)a, (const bf16*)x,
                       (const float*)mean, (const float*)rstd, w, w + C, rows, C, 128, count);
 }
-template <bool CENTRED>
 cudaError_t bn_fwd_apply(const void* x, const void* ws, const void* gamma, const void* beta, void* y, void* mean, void* rstd, int rows,
                          int C, float eps, int relu, float count, void* stream) {
   const float* w = (const float*)ws;
-  return tepd::launch(bn_fwd_apply_kernel<CENTRED>, dim3(grid_for((size_t)rows * C / 8, 256)), dim3(256), 0, CS(stream), (const bf16*)x,
+  return tepd::launch(bn_fwd_apply_kernel, dim3(grid_for((size_t)rows * C / 8, 256)), dim3(256), 0, CS(stream), (const bf16*)x,
                       w, w + C, (const float*)gamma, (const float*)beta, (bf16*)y, (float*)mean, (float*)rstd, rows, C, eps, relu, count);
 }
 }  // namespace
@@ -861,7 +840,7 @@ extern "C" int tepd_bn_fwd_nhwc(const void* x, const void* gamma, const void* be
   cudaError_t e = bn_reduce<2>(x, nullptr, nullptr, nullptr, ws, rows, C, (float)rows, stream);
   if (e == cudaSuccess) e = bn_reduce<3>(x, nullptr, nullptr, nullptr, ws, rows, C, (float)rows, stream);
   if (e != cudaSuccess) return (int)e;
-  return (int)bn_fwd_apply<true>(x, ws, gamma, beta, y, mean, rstd, rows, C, eps, relu, (float)rows, stream);
+  return (int)bn_fwd_apply(x, ws, gamma, beta, y, mean, rstd, rows, C, eps, relu, (float)rows, stream);
 }
 extern "C" int tepd_bn_bwd_nhwc(const void* dy, const void* x, const void* gamma, const void* mean, const void* rstd, void* dx,
                                 void* ws, int rows, int C, void* stream) {
@@ -880,11 +859,9 @@ extern "C" int tepd_bn_bwd_nhwc(const void* dy, const void* x, const void* gamma
 //             with the global mean), all-reduce ws[1], tepd_bn_fwd_apply_centred_nhwc.  Every shard shifts by the same mean,
 //             so the all-reduced ws[1] is the centred second moment of the whole batch.
 //   backward: tepd_bn_reduce_nhwc mode 1 (ws = [sum(dy), sum(dy * xhat)]), all-reduce ws, tepd_bn_bwd_apply_nhwc.
-// mode 0 (ws = [sum(x), sum(x^2)]) with tepd_bn_fwd_apply_nhwc is the one-pass forward, which cancels when |mean| >> std.
 extern "C" int tepd_bn_reduce_nhwc(const void* a, const void* x, const void* mean, const void* rstd, void* ws, int rows, int C, int mode,
                                    void* stream) {
   if (C % 8) return -2;
-  if (mode == 0) return (int)bn_reduce<0>(a, nullptr, nullptr, nullptr, ws, rows, C, 0.f, stream);
   if (mode == 1) return (int)bn_reduce<1>(a, x, mean, rstd, ws, rows, C, 0.f, stream);
   if (mode == 2) return (int)bn_reduce<2>(a, nullptr, nullptr, nullptr, ws, rows, C, 0.f, stream);
   return -3;
@@ -894,16 +871,11 @@ extern "C" int tepd_bn_centred_sq_nhwc(const void* x, void* ws, int rows, int C,
   if (C % 8) return -2;
   return (int)bn_reduce<3>(x, nullptr, nullptr, nullptr, ws, rows, C, count, stream);
 }
-extern "C" int tepd_bn_fwd_apply_nhwc(const void* x, const void* ws, const void* gamma, const void* beta, void* y, void* mean, void* rstd,
-                                      int rows, int C, float eps, int relu, float count, void* stream) {
-  if (C % 8) return -2;
-  return (int)bn_fwd_apply<false>(x, ws, gamma, beta, y, mean, rstd, rows, C, eps, relu, count, stream);
-}
 // ws = [sum(x), sum((x - mean)^2)] over the global batch of `count` rows
 extern "C" int tepd_bn_fwd_apply_centred_nhwc(const void* x, const void* ws, const void* gamma, const void* beta, void* y, void* mean,
                                               void* rstd, int rows, int C, float eps, int relu, float count, void* stream) {
   if (C % 8) return -2;
-  return (int)bn_fwd_apply<true>(x, ws, gamma, beta, y, mean, rstd, rows, C, eps, relu, count, stream);
+  return (int)bn_fwd_apply(x, ws, gamma, beta, y, mean, rstd, rows, C, eps, relu, count, stream);
 }
 extern "C" int tepd_bn_bwd_apply_nhwc(const void* dy, const void* x, const void* gamma, const void* mean, const void* rstd, const void* ws,
                                       void* dx, int rows, int C, float count, void* stream) {

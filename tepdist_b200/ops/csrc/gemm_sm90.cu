@@ -2,9 +2,8 @@
 // into register accumulators of two consumer warpgroups -> epilogue from the accumulator fragments (bias / GELU /
 // residual / fp32 split-K or stream-K reduction fused).  bf16 outputs, and the fp32 weight-gradient outputs, whose layout
 // TMA can address go through a swizzled shared-memory staging buffer and TMA stores (or TMA reduce-adds) that overlap the
-// next tile's MMAs; the other outputs are stored straight from the fragments.  bf16 operands, and e4m3 operands for the
-// MoE expert GEMMs
-// (tepd_gemm_fp8).  This is the device-op layer that replaces the reference's cuBLAS GemmThunk
+// next tile's MMAs; the other outputs are stored straight from the fragments.  Operands are bf16.  This is the
+// device-op layer that replaces the reference's cuBLAS GemmThunk
 // (reference: tensorflow/compiler/xla/service/gpu/gemm_thunk.cc, SURVEY §2.H K8).
 //
 //   D[b, M, N] = epilogue( alpha * A[b] (M x K)  *  B[b] (K x N) )
@@ -22,7 +21,7 @@ using namespace sm90;
 namespace {
 
 constexpr int BLOCK_M = 128;
-constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row (128 e4m3 elements for the fp8 kernel)
+constexpr int BLOCK_K = 64;   // 64 bf16 = 128 B = one swizzle row
 constexpr int NUM_THREADS = 384;  // warpgroups 0, 1: consumers (232 registers), warpgroup 2: TMA producer (40)
 constexpr int CONSUMER_REGS = 232, PRODUCER_REGS = 40;   // 2 x 128 x 232 + 128 x 40 = 384 x 168, the launch allocation
 constexpr int STORE_BOX = 64;     // TMA store box: 64 columns (128 B, one swizzle row) x 64 rows = 8 KB
@@ -43,9 +42,6 @@ struct GemmParams {
   int bias_bf16;
   void* D2;        // act 1: when set, D receives the pre-activation and D2 the activated value (saved for backward)
   const void* aux; // act 2: bf16 [b, M, N] pre-activation
-  const float* row_scale;  // fp8: per-row activation scale [b, M] (nullptr: none); multiplied with w_scale[b]
-  const float* w_scale;
-  long long bias_stride;   // bias batch stride (elements): 0 = one bias for every batch
   int stream_k;    // > 0: stream-K -- CTA c owns the contiguous range [c, c+1) * stream_k of the (tile, k-block) iteration
                    // space and flushes its accumulator with red.add at every tile boundary (fp32 accumulate outputs only):
                    // every SM gets the same number of k-blocks whatever the tile count (no wave quantisation)
@@ -159,10 +155,10 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, const GemmPara
                                               bool add_res) {
   if (add_bias) {
     if (p.bias_bf16) {
-      const float2 f = ldg_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.bias) + (long long)b * p.bias_stride + col);
+      const float2 f = ldg_bf16x2(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col);
       v0 += f.x; v1 += f.y;
     } else {
-      const float2 f = __ldg(reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.bias) + (long long)b * p.bias_stride + col));
+      const float2 f = __ldg(reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.bias) + col));
       v0 += f.x; v1 += f.y;
     }
   }
@@ -190,13 +186,13 @@ __device__ __forceinline__ void epilogue_pair(float v0, float v1, const GemmPara
   }
 }
 
-// One k-block (BLOCK_K = 128 bytes of K) of this warpgroup's 64 x BLOCK_N accumulator: four wgmma k-steps, each one
-// m64n256k16 (BLOCK_N = 256) or m64n128 (BLOCK_N = 128).  bf16 steps are k16, e4m3 steps k32: 32 bytes of K either way,
-// so the descriptors advance alike.  The B descriptor covers all BLOCK_N rows: K-major B rows follow each other in the
-// swizzled tile (SBO), MN-major B is BLOCK_N / 64 chunks of 64 columns LBO apart.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8>
+// One k-block (BLOCK_K = 128 bytes of K) of this warpgroup's 64 x BLOCK_N accumulator: four wgmma k-steps of 16 bf16
+// (32 bytes of K), each one m64n256k16 (BLOCK_N = 256) or m64n128k16 (BLOCK_N = 128).  The B descriptor covers all
+// BLOCK_N rows: K-major B rows follow each other in the swizzled tile (SBO), MN-major B is BLOCK_N / 64 chunks of 64
+// columns LBO apart.
+template <int BLOCK_N, bool A_MN, bool B_MN>
 __device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 2], uint32_t sa, uint32_t sb, int wg, bool first) {
-  static_assert(BLOCK_N == 128 || (BLOCK_N == 256 && !FP8), "tile width");
+  static_assert(BLOCK_N == 128 || BLOCK_N == 256, "tile width");
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     uint64_t da, db;
@@ -205,15 +201,14 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BLOCK_N / 2], uint32_t s
     if constexpr (!B_MN) db = make_smem_desc_sw128(sb + k * 32, 0, 1024);
     else                 db = make_smem_desc_sw128(sb + k * 16 * 128, 64 * BLOCK_K * 2, 1024);
     const uint32_t scale_d = (first && k == 0) ? 0u : 1u;
-    if constexpr (FP8)                 wgmma_m64n128k32_e4m3_ss(acc, da, db, scale_d);
-    else if constexpr (BLOCK_N == 256) wgmma_m64n256k16_bf16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, scale_d);
-    else                               wgmma_m64n128k16_bf16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, scale_d);
+    if constexpr (BLOCK_N == 256) wgmma_m64n256k16_bf16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, scale_d);
+    else                          wgmma_m64n128k16_bf16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, scale_d);
   }
 }
 
 // Warp roles: warpgroups 0, 1 = consumers (wgmma into registers, rows [64 wg, +64) of the 128-row tile, then the
 // epilogue); warpgroup 2 = TMA producer (one elected thread), which hands most of its registers to the consumers.
-template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8, int EPI>
+template <int BLOCK_N, bool A_MN, bool B_MN, int EPI>
 __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap& tmap_d,
                                           const CUtensorMap& tmap_d2, const CUtensorMap& tmap_in, const GemmParams& p) {
   constexpr bool STAGED = EPI != EPI_DIRECT;
@@ -267,7 +262,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
           uint8_t* sb = sa + C::A_BYTES;
           mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
           if constexpr (!A_MN) {
-            tma_load_3d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K * (FP8 ? 2 : 1), a_row, b);
+            tma_load_3d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, a_row, b);
           } else {
 #pragma unroll
             for (int j = 0; j < BLOCK_M / 64; ++j)
@@ -275,7 +270,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
                           m_blk * BLOCK_M + j * 64, kb * BLOCK_K, b);
           }
           if constexpr (!B_MN) {
-            tma_load_3d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K * (FP8 ? 2 : 1), n_blk * BLOCK_N, b);
+            tma_load_3d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, n_blk * BLOCK_N, b);
           } else {
 #pragma unroll
             for (int j = 0; j < BLOCK_N / 64; ++j)
@@ -317,7 +312,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
             float v = 0.f;
             if (p.bias != nullptr && col < p.N)
               v = p.bias_bf16 ? __bfloat162float(__ldg(reinterpret_cast<const __nv_bfloat16*>(p.bias) + col))
-                              : __ldg(reinterpret_cast<const float*>(p.bias) + col);   // (bias_stride is 0 here)
+                              : __ldg(reinterpret_cast<const float*>(p.bias) + col);
             sbias[c] = v;
           }
         }
@@ -338,7 +333,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * C::STAGE_BYTES);
         wgmma_fence();
-        mma_kblock<BLOCK_N, A_MN, B_MN, FP8>(acc, sa, sa + C::A_BYTES, wg, kb == w.kb0);
+        mma_kblock<BLOCK_N, A_MN, B_MN>(acc, sa, sa + C::A_BYTES, wg, kb == w.kb0);
         wgmma_commit();
         wgmma_wait<1>();   // the previous k-block's MMAs have retired: its slot may be refilled
         if (prev >= 0 && t128 == 0) mbar_arrive(&empty_bar[prev]);
@@ -432,18 +427,15 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
         continue;
       }
       if (has_k) {
-        const float* scale_rows = p.row_scale ? p.row_scale + (long long)b * p.M : nullptr;
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
           const int row = m_blk * BLOCK_M + row_base + hr * 8;
           if (row >= p.M) continue;
-          float alpha = p.alpha;
-          if (scale_rows) alpha *= scale_rows[row] * p.w_scale[b];
 #pragma unroll
           for (int j = 0; j < BLOCK_N / 8; ++j) {
             const int col = n_blk * BLOCK_N + j * 8 + 2 * q;
             if (col >= p.N) continue;
-            epilogue_pair(acc[4 * j + 2 * hr] * alpha, acc[4 * j + 2 * hr + 1] * alpha, p, row, col, b, add_bias, add_res);
+            epilogue_pair(acc[4 * j + 2 * hr] * p.alpha, acc[4 * j + 2 * hr + 1] * p.alpha, p, row, col, b, add_bias, add_res);
           }
         }
       }
@@ -454,12 +446,12 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
   }
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8, int EPI>
+template <int BLOCK_N, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_d2,
                  const __grid_constant__ CUtensorMap tmap_in, const GemmParams p) {
-  gemm_body<BLOCK_N, A_MN, B_MN, FP8, EPI>(tmap_a, tmap_b, tmap_d, tmap_d2, tmap_in, p);
+  gemm_body<BLOCK_N, A_MN, B_MN, EPI>(tmap_a, tmap_b, tmap_d, tmap_d2, tmap_in, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -511,10 +503,10 @@ extern "C" int tepd_make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, long lo
 
 struct Maps { CUtensorMap a, b, d, d2, in; };
 
-template <int BLOCK_N, bool A_MN, bool B_MN, bool FP8, int EPI>
+template <int BLOCK_N, bool A_MN, bool B_MN, int EPI>
 static int launch_gemm(const Maps& m, const GemmParams& p, int num_sms, cudaStream_t stream) {
   using C = Cfg<BLOCK_N, EPI != EPI_DIRECT>;
-  auto kern = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, FP8, EPI>;
+  auto kern = gemm_bf16_kernel<BLOCK_N, A_MN, B_MN, EPI>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
@@ -571,7 +563,6 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
   p.D = D; p.bias = bias; p.residual = residual; p.alpha = alpha;
   p.out_fp32 = out_fp32; p.accumulate = accumulate; p.act = act; p.bias_bf16 = bias_bf16;
   p.D2 = D2; p.aux = aux;
-  p.row_scale = nullptr; p.w_scale = nullptr; p.bias_stride = 0;
 
   CUtensorMap ta, tb;
   int rc;
@@ -614,54 +605,23 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
     if (rc) return 300 + rc;
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-#define LAYOUTS(BN, E)                                                                \
-  if (!a_mn && !b_mn) return launch_gemm<BN, false, false, false, E>(m, p, num_sms, s); \
-  if (!a_mn && b_mn) return launch_gemm<BN, false, true, false, E>(m, p, num_sms, s);   \
-  if (a_mn && !b_mn) return launch_gemm<BN, true, false, false, E>(m, p, num_sms, s);   \
-  return launch_gemm<BN, true, true, false, E>(m, p, num_sms, s);
-#define KINDS(BN)                                                                                         \
-  switch (epi) {                                                                                          \
-    case EPI_PLAIN: { LAYOUTS(BN, EPI_PLAIN) }                                                            \
-    case EPI_BIAS: return launch_gemm<BN, false, false, false, EPI_BIAS>(m, p, num_sms, s);               \
-    case EPI_BIAS_RES: return launch_gemm<BN, false, false, false, EPI_BIAS_RES>(m, p, num_sms, s);       \
-    case EPI_GELU_DUAL: return launch_gemm<BN, false, false, false, EPI_GELU_DUAL>(m, p, num_sms, s);     \
-    case EPI_GELU_BWD: return launch_gemm<BN, false, true, false, EPI_GELU_BWD>(m, p, num_sms, s);        \
-    case EPI_F32: return launch_gemm<BN, true, true, false, EPI_F32>(m, p, num_sms, s);                   \
-    case EPI_F32_ADD: return launch_gemm<BN, true, true, false, EPI_F32_ADD>(m, p, num_sms, s);           \
-    default: { LAYOUTS(BN, EPI_DIRECT) }                                                                  \
+#define LAYOUTS(BN, E)                                                         \
+  if (!a_mn && !b_mn) return launch_gemm<BN, false, false, E>(m, p, num_sms, s); \
+  if (!a_mn && b_mn) return launch_gemm<BN, false, true, E>(m, p, num_sms, s);   \
+  if (a_mn && !b_mn) return launch_gemm<BN, true, false, E>(m, p, num_sms, s);   \
+  return launch_gemm<BN, true, true, E>(m, p, num_sms, s);
+#define KINDS(BN)                                                                                  \
+  switch (epi) {                                                                                   \
+    case EPI_PLAIN: { LAYOUTS(BN, EPI_PLAIN) }                                                     \
+    case EPI_BIAS: return launch_gemm<BN, false, false, EPI_BIAS>(m, p, num_sms, s);               \
+    case EPI_BIAS_RES: return launch_gemm<BN, false, false, EPI_BIAS_RES>(m, p, num_sms, s);       \
+    case EPI_GELU_DUAL: return launch_gemm<BN, false, false, EPI_GELU_DUAL>(m, p, num_sms, s);     \
+    case EPI_GELU_BWD: return launch_gemm<BN, false, true, EPI_GELU_BWD>(m, p, num_sms, s);        \
+    case EPI_F32: return launch_gemm<BN, true, true, EPI_F32>(m, p, num_sms, s);                   \
+    case EPI_F32_ADD: return launch_gemm<BN, true, true, EPI_F32_ADD>(m, p, num_sms, s);           \
+    default: { LAYOUTS(BN, EPI_DIRECT) }                                                           \
   }
   if (block_n == 256) { KINDS(256) } else { KINDS(128) }
 #undef KINDS
 #undef LAYOUTS
-}
-
-// ------------------------------------------------------------------ fp8 (e4m3) grouped GEMM for the MoE experts
-static int make_tmap_u8(CUtensorMap* out, const void* ptr, long long inner, long long rows, long long batch, int box_rows) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return -1;
-  cuuint64_t dims[3] = {(cuuint64_t)inner, (cuuint64_t)rows, (cuuint64_t)batch};
-  cuuint64_t strides[2] = {(cuuint64_t)inner, (cuuint64_t)(inner * rows)};
-  cuuint32_t box[3] = {128, (cuuint32_t)box_rows, 1}, es[3] = {1, 1, 1};
-  return fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS ? 0 : -2;
-}
-
-// D[b] (bf16 [M,N]) = act((A[b] (e4m3 [M,K]) . B[b]^T (e4m3 [N,K])) * row_scale[b,:] * w_scale[b] + bias[b])
-extern "C" int tepd_gemm_fp8(const void* A, const void* B, void* D, const void* row_scale, const void* w_scale, const void* bias, int M,
-                             int N, int K, int batch, int act, int num_sms, void* stream) {
-  if (K % 16 || N % 8 || M <= 0) return -2;
-  constexpr int BN = 128;
-  GemmParams p;
-  p.M = M; p.N = N; p.K = K; p.batch = batch;
-  p.m_blocks = (M + BLOCK_M - 1) / BLOCK_M; p.n_blocks = (N + BN - 1) / BN; p.k_blocks = (K + 127) / 128;
-  p.split_k = 1; p.stream_k = 0;
-  p.ldd = N; p.stride_d = (long long)M * N; p.ld_res = 0; p.stride_res = 0;
-  p.D = D; p.bias = bias; p.residual = nullptr; p.alpha = 1.0f;
-  p.out_fp32 = 0; p.accumulate = 0; p.act = act == 1 ? 1 : 0; p.bias_bf16 = 0; p.D2 = nullptr; p.aux = nullptr;
-  p.row_scale = (const float*)row_scale; p.w_scale = (const float*)w_scale; p.bias_stride = N;
-  Maps m;
-  m.d = m.d2 = m.in = CUtensorMap{};
-  if (make_tmap_u8(&m.a, A, K, M, batch, BLOCK_M) || make_tmap_u8(&m.b, B, K, N, batch, BN)) return -3;
-  if (num_sms <= 0) num_sms = tepd::num_sms();
-  return launch_gemm<BN, false, false, true, EPI_DIRECT>(m, p, num_sms, reinterpret_cast<cudaStream_t>(stream));
 }

@@ -1,5 +1,5 @@
 """Element-by-element numerics of the kernels one Wide-ResNet training step launches (convolution, BatchNorm, pooling, the
-conv-net elementwise ops, SGD, axpy), and every parameter's gradient of whole Wide-ResNet steps against the fp32 CPU executor.
+conv-net elementwise ops, SGD), and every parameter's gradient of whole Wide-ResNet steps against the fp32 CPU executor.
 
 Conventions as in test_step_numerics_gpu.py: every case checks that our kernel ran, and compares each element with a
 reference computed in fp64 from the same bf16 / fp32 inputs; bit for bit where the arithmetic is exact, otherwise within a
@@ -295,7 +295,7 @@ def test_batchnorm_split_phases_one_gpu(ops, C, N, H, W, shards):
         close(f"dbeta of shard {s}", db, db_ref, t_db)
 
 
-# ============================================================================================== C. pooling, elementwise, SGD, axpy
+# ============================================================================================== C. pooling, elementwise, SGD
 def maxpool_ref(x, dy, k, s, p):
     """fp64 max pool and its gradient with the first maximum of a window (row-major scan) taking dy, on -inf padding."""
     N, C, H, W = x.shape
@@ -388,26 +388,6 @@ def test_sgd_step(ops, with_copy):
     close("sgd", p, ref, 2 * (U32 * ref.abs() + 2 * U32 * upd.abs()) + FTZ)
     if with_copy:
         exact("sgd bf16 copy", pb, p.to(torch.bfloat16))
-
-
-def test_axpy_f32(ops):
-    """acc + a g (one product and one addition, possibly an FMA): within u |acc'| + u |a g|, doubled.  n % 4 != 0 is
-    refused before any launch and leaves acc untouched."""
-    _seed(42)
-    n, a = 4 * 250_001, 0.3
-    acc0 = torch.randn(n, device="cuda", generator=gen())
-    g = torch.randn(n, device="cuda", generator=gen()) * 5
-    acc = acc0.clone()
-    launched(ops, ops.axpy_f32, acc, g, a)
-    ag = float(torch.tensor(a, dtype=torch.float32)) * g.double()
-    ref = acc0.double() + ag
-    close("axpy", acc, ref, 2 * (U32 * ref.abs() + U32 * ag.abs()) + FTZ)
-    bad = acc0[:n - 2].clone()
-    n0 = ops.launch_count()
-    with pytest.raises(RuntimeError, match="axpy_f32"):
-        ops.axpy_f32(bad, g[:n - 2], a)
-    assert ops.launch_count() == n0
-    assert torch.equal(bad, acc0[:n - 2])
 
 
 # ============================================================================================== D. whole Wide-ResNet steps

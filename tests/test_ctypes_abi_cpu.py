@@ -1,5 +1,5 @@
 """The Python side talks to the CUDA library through hand-written ctypes argtypes tables (ops/__init__.py `_Sig`,
-parallel/symm.py `_sigs` / `_vmm_sigs`, parallel/moe.py `_sig`).  A mismatch in COUNT or KIND against the `extern "C"`
+parallel/symm.py `_sigs` / `_vmm_sigs`).  A mismatch in COUNT or KIND against the `extern "C"`
 declaration does not fail loudly -- arguments are just reinterpreted.  This test parses every `extern "C" int tepd_*(...)`
 in ops/csrc/*.cu and compares it parameter by parameter with what the Python modules install.  Static check only: it says
 nothing about whether the VALUES passed at the call sites are the right ones."""
@@ -75,19 +75,18 @@ class _FakeLib:
 
 def _python_tables():
     from tepdist_b200 import ops
-    from tepdist_b200.parallel import moe, symm
+    from tepdist_b200.parallel import symm
     tables = {n: getattr(ops._Sig, n) for n in dir(ops._Sig) if n.startswith("tepd_")}
     lib = _FakeLib()
     symm._sigs(lib)
     symm._vmm_sigs(lib)
-    moe._sig(lib)
     for name, fn in lib.fns.items():
         assert name not in tables, f"{name} has two argtypes tables"
         tables[name] = fn.argtypes
     return tables
 
 
-def test_every_ctypes_table_matches_its_extern_c_declaration():
+def test_every_ctypes_table_matches_its_c_declaration():
     decls, tables = _c_decls(), _python_tables()
     assert len(decls) >= 35, sorted(decls)
     problems = []
@@ -106,7 +105,7 @@ def test_every_ctypes_table_matches_its_extern_c_declaration():
     assert not problems, "\n".join(problems)
 
 
-def test_every_kernel_entry_point_used_from_python_has_a_table():
+def test_every_kernel_entry_point_has_a_ctypes_table():
     """Entry points without an argtypes table would be called with ctypes' default int conversion (truncates 64-bit pointers)."""
     decls, tables = _c_decls(), _python_tables()
     internal = {"tepd_make_tmap_bf16_3d", "tepd_make_tmap_bshd", "tepd_make_tmap_3d"}       # called from C++ only

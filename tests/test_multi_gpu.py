@@ -26,17 +26,6 @@ def test_fused_dp_matches_nccl_and_single(tmp_path):
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
-def test_fused_moe_expert_parallel_fp8(tmp_path):
-    out = str(tmp_path / "moe.json")
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
-           "--master-port", "29743", os.path.join(HERE, "moe_fused_worker.py"), out]
-    pr = subprocess.run(cmd, capture_output=True, text=True, timeout=600)
-    assert pr.returncode == 0, pr.stderr[-3000:]
-    r = json.load(open(out))
-    assert r["relerr"] < 6e-2, r          # e4m3 activations x e4m3 weights
-
-
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_tp_plan_fused_all_reduce_matches_nccl(tmp_path):
     out = str(tmp_path / "tpplan.json")
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
