@@ -320,6 +320,17 @@ def ew_native(mode: str, a: torch.Tensor, b: Optional[torch.Tensor] = None) -> O
 
 
 # --------------------------------------------------------------------------------------------- MoE route-table kernels
+# The kernels index with the route tables as given: an int32 table, an fp32 weight and shapes that match the data operand
+# are checked here, before any launch.  Each `.contiguous()` copy is bound to a local that lives until the launch has been
+# enqueued: a temporary freed after `.data_ptr()` goes back to the caching allocator, and the next operand's copy of the
+# same byte size would be placed at the same address.
+def _route_tables(what: str, shape, **tables: torch.Tensor) -> None:
+    for name, t in tables.items():
+        want = torch.float32 if name in ("w", "gw") else torch.int32
+        if t.dtype != want or tuple(t.shape) != tuple(shape):
+            raise ValueError(f"{what}: {name} must be {want} of shape {tuple(shape)}; got {t.dtype} {tuple(t.shape)}")
+
+
 def moe_gather_scale(src: torch.Tensor, slot_src: torch.Tensor, w: torch.Tensor, E: int, C: int) -> torch.Tensor:
     """out[e, g, c, :] = w[g, e, c] * src[g, slot_src[g, e, c], :] (zero where slot_src < 0).  src [G, S, M]; slot_src int32 [G, E, C]."""
     G, S, M = src.shape
@@ -329,9 +340,11 @@ def moe_gather_scale(src: torch.Tensor, slot_src: torch.Tensor, w: torch.Tensor,
         rows = torch.gather(src.float(), 1, idx.unsqueeze(-1).expand(G, E * C, M)).reshape(G, E, C, M)
         out = rows * (w.float() * valid).unsqueeze(-1)
         return out.permute(1, 0, 2, 3).contiguous().to(src.dtype)
+    _route_tables("moe_gather_scale", (G, E, C), slot_src=slot_src, w=w)
+    src_c, slot_c, w_c = src.contiguous(), slot_src.contiguous(), w.contiguous()
     out = torch.empty(E, G, C, M, dtype=src.dtype, device=src.device)
-    _check(lib().tepd_moe_gather_scale(src.contiguous().data_ptr(), slot_src.contiguous().data_ptr(), w.contiguous().data_ptr(),
-                                       out.data_ptr(), G, S, E, C, M, _stream()), "moe_gather_scale")
+    _check(lib().tepd_moe_gather_scale(src_c.data_ptr(), slot_c.data_ptr(), w_c.data_ptr(), out.data_ptr(), G, S, E, C, M,
+                                       _stream()), "moe_gather_scale")
     _count()
     return out
 
@@ -346,9 +359,11 @@ def moe_combine_sum(y: torch.Tensor, re: torch.Tensor, rc: torch.Tensor, gw: tor
         rows = torch.gather(yg, 1, flat.unsqueeze(-1).expand(G, S * K, M)).reshape(G, S, K, M)
         out = (rows * (gw.float() * (re >= 0)).unsqueeze(-1)).sum(2)
         return out.to(y.dtype)
+    _route_tables("moe_combine_sum", (G, S, K), re=re, rc=rc, gw=gw)
+    y_c, re_c, rc_c, gw_c = y.contiguous(), re.contiguous(), rc.contiguous(), gw.contiguous()
     out = torch.empty(G, S, M, dtype=y.dtype, device=y.device)
-    _check(lib().tepd_moe_combine_sum(y.contiguous().data_ptr(), re.contiguous().data_ptr(), rc.contiguous().data_ptr(),
-                                      gw.contiguous().data_ptr(), out.data_ptr(), G, S, E, C, M, K, _stream()), "moe_combine_sum")
+    _check(lib().tepd_moe_combine_sum(y_c.data_ptr(), re_c.data_ptr(), rc_c.data_ptr(), gw_c.data_ptr(), out.data_ptr(), G, S, E,
+                                      C, M, K, _stream()), "moe_combine_sum")
     _count()
     return out
 
@@ -363,9 +378,13 @@ def moe_route_dots(a: torch.Tensor, b: torch.Tensor, re: torch.Tensor, rc: torch
         flat = (re.clamp(min=0).long() * C + rc.clamp(min=0).long()).reshape(G, S * K)
         rows = torch.gather(bg, 1, flat.unsqueeze(-1).expand(G, S * K, M)).reshape(G, S, K, M)
         return ((rows * a.float().unsqueeze(2)).sum(-1) * (re >= 0)).float()
+    if tuple(b.shape) != (E, G, C, M):
+        raise ValueError(f"moe_route_dots: b must be [E, G, C, M] = {(E, G, C, M)} for a {tuple(a.shape)}; got {tuple(b.shape)}")
+    _route_tables("moe_route_dots", (G, S, K), re=re, rc=rc)
+    a_c, b_c, re_c, rc_c = a.contiguous(), b.contiguous(), re.contiguous(), rc.contiguous()
     dots = torch.empty(G, S, K, dtype=torch.float32, device=a.device)
-    _check(lib().tepd_moe_route_dots(a.contiguous().data_ptr(), b.contiguous().data_ptr(), re.contiguous().data_ptr(),
-                                     rc.contiguous().data_ptr(), dots.data_ptr(), G, S, E, C, M, K, _stream()), "moe_route_dots")
+    _check(lib().tepd_moe_route_dots(a_c.data_ptr(), b_c.data_ptr(), re_c.data_ptr(), rc_c.data_ptr(), dots.data_ptr(), G, S, E, C,
+                                     M, K, _stream()), "moe_route_dots")
     _count()
     return dots
 
@@ -503,8 +522,9 @@ def global_avgpool_bwd(dy: torch.Tensor, shape) -> torch.Tensor:
     N, C, H, W = shape
     if not (CONV_NATIVE and dy.is_cuda and dy.dtype == torch.bfloat16 and C % 8 == 0):
         return (dy / (H * W)).view(N, C, 1, 1).expand(N, C, H, W).contiguous()
+    dy = dy.contiguous()     # (a local: the copy must outlive the launch, see the MoE wrappers)
     dx = torch.empty((N, C, H, W), dtype=dy.dtype, device=dy.device, memory_format=torch.channels_last)
-    _check(lib().tepd_gap_bwd_nhwc(dy.contiguous().data_ptr(), dx.data_ptr(), N, H * W, C, _stream()), "gap_bwd")
+    _check(lib().tepd_gap_bwd_nhwc(dy.data_ptr(), dx.data_ptr(), N, H * W, C, _stream()), "gap_bwd")
     _count()
     return dx
 
@@ -619,10 +639,10 @@ def layernorm_bwd(dy, x, gamma, mean, rstd, dgamma_acc: torch.Tensor, dbeta_acc:
             dx = dx + dres.float().reshape(rows, C)
         return dx.to(x.dtype).reshape(x.shape)
     dy = dy.contiguous()
+    dres = None if dres is None else dres.contiguous()     # (a local: the copy must outlive the launch, see the MoE wrappers)
     dx = torch.empty_like(x)
     _check(lib().tepd_layernorm_bwd(dy.data_ptr(), x.data_ptr(), gamma.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
-                                    dx.data_ptr(), dgamma_acc.data_ptr(), dbeta_acc.data_ptr(),
-                                    None if dres is None else dres.contiguous().data_ptr(), rows, C, _stream()),
+                                    dx.data_ptr(), dgamma_acc.data_ptr(), dbeta_acc.data_ptr(), _p(dres), rows, C, _stream()),
            "layernorm_bwd")
     _count()
     return dx

@@ -1080,6 +1080,20 @@ class Executor:
         elif kind == "sgd":
             ops.sgd_step(st.master, st.grad, st.compute, self._lr(1e-2))
 
+    def _moe_choices(self, n: Node, gates: torch.Tensor) -> torch.Tensor:
+        """Top-k expert choice of moe_dispatch_mask / moe_dispatch_mask_bwd node `n`: round r takes each token's r-th largest
+        gate, the lowest expert index on ties.  -> int64 [G, S, k].  Slot positions, capacity drops and the route tables follow
+        from these choices and the gate values; the fp32 oracle of a bf16 step is given the GPU's choices through this method,
+        because gates that nearly tie pick different experts at the two precisions."""
+        k = int(n.attrs.get("top_k", 2))
+        remaining = gates.clone()
+        out = []
+        for _ in range(k):
+            idx = remaining.argmax(-1)
+            out.append(idx)
+            remaining = remaining.masked_fill(torch.nn.functional.one_hot(idx, gates.shape[-1]).bool(), float("-inf"))
+        return torch.stack(out, -1)
+
     @staticmethod
     def _find_moe_einsums(g: Graph) -> Dict[int, Tuple[str, int]]:
         """einsum node id -> (kind, id of the moe_dispatch_mask node whose route tables it can use).  Matches the GShard
@@ -1519,12 +1533,12 @@ class Executor:
             gates = (ins[0] if op == "moe_dispatch_mask" else ins[1]).float()
             C, k = int(a["capacity"]), int(a.get("top_k", 2))
             Gn, Sn, E = gates.shape
-            remaining = gates.clone()
+            choices = self._moe_choices(n, gates)
             offset = torch.zeros(Gn, 1, E, device=gates.device)
             sel = torch.zeros(Gn, Sn, E, C, device=gates.device)   # 0/1 slot assignment
             r_e, r_c, r_w = [], [], []
-            for _ in range(k):
-                idx = remaining.argmax(-1)
+            for r in range(k):
+                idx = choices[..., r]
                 mask = F.one_hot(idx, E).float()
                 pos = (mask.cumsum(1) - 1 + offset) * mask
                 keep = (pos < C).float() * mask
@@ -1535,7 +1549,6 @@ class Executor:
                     r_c.append((pos * mask).sum(-1).long().clamp(max=C - 1).int())
                     r_w.append(gates.gather(-1, idx.unsqueeze(-1)).squeeze(-1) * kept)
                 offset = offset + mask.sum(1, keepdim=True)
-                remaining = remaining.masked_fill(mask.bool(), float("-inf"))
             if op == "moe_dispatch_mask":
                 out = (gates.unsqueeze(-1) * sel).to(torch_dtype(n.outputs[0].dtype, self.device))
                 if MOE_SPARSE:

@@ -1,6 +1,7 @@
 """GPU numerics of the flash-attention kernels at 64-wide heads (the GPT-2 345M head width), element by element against an
 fp64 autograd reference: the 345M shape with q / k / v as views of one fused [B, S, H, 3, D] buffer (as the executor passes
-them), a single tile, a long causal row, a non-causal shape with an odd head count, and the dqkv_out path.  A second call
+them), a single tile, a long causal row, a non-causal shape with an odd head count, the GPT-MoE shape with 48-wide heads
+(16 x 48 = 768, zero-padded onto the D = 64 kernels), and the dqkv_out path.  A second call
 must reproduce O, lse, dK and dV bit for bit; dQ is summed over KV blocks with fp32 reduce-adds whose order may differ.
 Every case checks that our kernels ran: the launch counter grows and the torch-math attention paths are errors."""
 import pytest
@@ -8,7 +9,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-D = 64
+D = 64     # (the head width unless a case gives another)
 
 
 def _kernels_only(monkeypatch):
@@ -25,7 +26,7 @@ def _kernels_only(monkeypatch):
     return ops
 
 
-def _inputs(B, S, H, seed):
+def _inputs(B, S, H, seed, D=D):
     g = torch.Generator(device="cuda").manual_seed(seed)
     qkv = torch.randn(B, S, H, 3, D, device="cuda", generator=g).to(torch.bfloat16)
     do = torch.randn(B, S, H, D, device="cuda", generator=g).to(torch.bfloat16)
@@ -34,7 +35,7 @@ def _inputs(B, S, H, seed):
 
 def _ref(q, k, v, do, causal):
     """fp64 autograd attention on [B, S, H, D] -> (o, lse [B, H, S], dq, dk, dv)."""
-    S = q.shape[1]
+    S, D = q.shape[1], q.shape[3]
     qf, kf, vf = (t.double().detach().clone().requires_grad_(True) for t in (q, k, v))
     s = torch.einsum("bqhd,bkhd->bhqk", qf, kf) * D ** -0.5
     if causal:
@@ -63,15 +64,19 @@ def _run(ops, q, k, v, do, causal, dqkv_out=None):
     return [t.clone() for t in (o, lse, dq, dk, dv)]
 
 
-@pytest.mark.parametrize("B,S,H,causal", [
-    (4, 1024, 16, True),    # GPT-2 345M
-    (2, 128, 2, True),
-    (1, 4096, 2, True),
-    (2, 512, 3, False),
-])
-def test_hd64_matches_fp64_reference_and_repeats(B, S, H, causal, monkeypatch):
+CASES = [
+    (4, 1024, 16, True, 64),    # GPT-2 345M
+    (2, 128, 2, True, 64),
+    (1, 4096, 2, True, 64),
+    (2, 512, 3, False, 64),
+    (2, 1024, 16, True, 48),    # GPT-MoE: 16 heads x 48
+]
+
+
+@pytest.mark.parametrize("B,S,H,causal,D", CASES, ids=["-".join(map(str, c[:4])) + ("" if c[4] == D else f"-D{c[4]}") for c in CASES])
+def test_hd64_matches_fp64_reference_and_repeats(B, S, H, causal, D, monkeypatch):
     ops = _kernels_only(monkeypatch)
-    q, k, v, do = _inputs(B, S, H, seed=S + H)
+    q, k, v, do = _inputs(B, S, H, seed=S + H, D=D)
     first = _run(ops, q, k, v, do, causal)
     o, lse, dq, dk, dv = first
     o_ref, lse_ref, *g_ref = _ref(q, k, v, do, causal)
