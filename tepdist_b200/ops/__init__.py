@@ -96,6 +96,7 @@ class _Sig:
     tepd_xent_fwd_bwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp]
     tepd_adamw = [_vp, _vp, _vp, _vp, _vp, _ll, _ll, _f, _f, _f, _f, _f, _f, _f, _f, _vp, _vp]
     tepd_sgd = [_vp, _vp, _vp, _ll, _f, _f, _vp]
+    tepd_optim_step = [_i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
     tepd_cast_f32_bf16 = [_vp, _vp, _ll, _vp]
     tepd_ew_bf16 = [_vp, _vp, _vp, _ll, _i, _vp]
     tepd_moe_gather_scale = [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]
@@ -812,6 +813,137 @@ def sgd_step(p: torch.Tensor, g: torch.Tensor, p_bf16: Optional[torch.Tensor], l
         return
     _check(lib().tepd_sgd(p.data_ptr(), g.data_ptr(), _p(p_bf16), p.numel(), lr, grad_scale, _stream()), "sgd")
     _count()
+
+
+# Multi-tensor updates of the optimizers with per-variable reductions (runtime/optimizers.py is their specification;
+# optim_sm90.cu the kernels).  The work table is built once per plan; each step is a fixed number of launches per kind.
+OPTIM_KINDS = {"apply_momentum": 0, "apply_lamb": 1, "apply_adafactor": 2, "apply_sm3": 3}
+OPTIM_LAUNCHES = {"apply_momentum": 1, "apply_lamb": 2, "apply_adafactor": 4, "apply_sm3": 2}
+OPTIM_FLAT_CHUNK = 16384      # elements per chunk of an elementwise-chunked variable (a multiple of 4)
+OPTIM_ROW_CHUNK = 32          # rows per chunk of a row-chunked variable (kWarps * kRowsPerWarp in optim_sm90.cu)
+_OPT_DECAY, _OPT_ROWS, _OPT_MOM = 1, 2, 4
+
+
+def optim_slot_shapes(op: str, shape, opt) -> Optional[list]:
+    """Slot shapes the multi-tensor kernels expect for a variable of `shape` (those frontend.builder.apply_optimizer gives),
+    or None when the kernels do not cover the variable (SM3 above rank 3, empty variables)."""
+    shape = tuple(shape)
+    if not shape or math.prod(shape) == 0:
+        return None
+    if op == "apply_momentum":
+        return [shape]
+    if op == "apply_lamb":
+        return [shape, shape]
+    if op == "apply_adafactor":
+        if len(shape) >= 2 and opt.get("factored", True):
+            return [shape[:-1], shape[:-2] + shape[-1:]]
+        return [shape]
+    if op == "apply_sm3":
+        if len(shape) > 3:
+            return None
+        accs = [(d,) for d in shape] if len(shape) > 1 else [shape]
+        return accs + ([shape] if opt.get("momentum", 0.0) > 0 else [])
+    return None
+
+
+def optim_tables(op: str, shapes, offsets, decays, opt):
+    """Host work table of one multi-tensor update (layouts OptVar / OptChunk in optim_sm90.cu, slot pointers left 0).
+    -> (vars int64 [V, 16], chunks int64 [N, 6], work-space floats, col_blocks).  Row-chunked (Adafactor factored, SM3
+    rank >= 2) variables are cut into OPTIM_ROW_CHUNK whole rows of their [B * R, C] view, the others into flat chunks."""
+    import numpy as np
+    vars_ = np.zeros((len(shapes), 16), dtype=np.int64)
+    chunks = []
+    nchunks = 0
+    col_blocks = 1
+    extra = []          # (var, floats) of the work space after the per-chunk partials
+    for i, (shape, off, decay) in enumerate(zip(shapes, offsets, decays)):
+        shape = tuple(int(d) for d in shape)
+        n = math.prod(shape)
+        rows = len(shape) >= 2 and ((op == "apply_adafactor" and opt.get("factored", True)) or op == "apply_sm3")
+        if rows:
+            B, R, C = math.prod(shape[:-2]), shape[-2], shape[-1]
+            cpb = -(-R // OPTIM_ROW_CHUNK)
+            r0 = np.arange(cpb, dtype=np.int64) * OPTIM_ROW_CHUNK
+            nr = np.minimum(OPTIM_ROW_CHUNK, R - r0)
+            for b in range(B):
+                c = np.zeros((cpb, 6), dtype=np.int64)
+                c[:, 0], c[:, 1], c[:, 2], c[:, 3] = i, b, r0, nr
+                c[:, 4], c[:, 5] = (b * R + r0) * C, nr * C
+                chunks.append(c)
+            nc = B * cpb
+            extra.append((i, nc * C if op == "apply_adafactor" else B + R + C))
+            col_blocks = max(col_blocks, -(-(B * C if op == "apply_adafactor" else B + R + C) // 256))
+        else:
+            B, R, C, cpb = 1, 1, n, 0
+            e0 = np.arange(0, n, OPTIM_FLAT_CHUNK, dtype=np.int64)
+            c = np.zeros((len(e0), 6), dtype=np.int64)
+            c[:, 0], c[:, 4], c[:, 5] = i, e0, np.minimum(OPTIM_FLAT_CHUNK, n - e0)
+            chunks.append(c)
+            nc = len(e0)
+        flags = (_OPT_DECAY if decay else 0) | (_OPT_ROWS if rows else 0)
+        if op == "apply_sm3" and opt.get("momentum", 0.0) > 0:
+            flags |= _OPT_MOM
+        vars_[i, :11] = (off, n, B, R, C, flags, nchunks, nc, 0, len(shape), 0)
+        vars_[i, 14] = cpb
+        nchunks += nc
+    ws = 4 * nchunks
+    for i, size in extra:
+        vars_[i, 8] = ws
+        ws += size
+    return vars_, np.concatenate(chunks), ws, min(col_blocks, 1024)
+
+
+class OptimPlan:
+    """One multi-tensor optimizer update over whole variables of the flat buffers.  `variables`: [(flat offset, shape,
+    slot tensors, decay)] with the slots optim_slot_shapes names, contiguous fp32.  On CUDA the work table (and the
+    kernels' work space) is built here once; a CPU plan keeps only the list, optim_step then runs runtime/optimizers.py."""
+
+    def __init__(self, op: str, opt: dict, variables, device: torch.device):
+        self.op, self.opt, self.variables = op, dict(opt), list(variables)
+        self.launches = OPTIM_LAUNCHES[op]
+        self.device = device
+        if device.type != "cuda":
+            return
+        shapes = [s for _, s, _, _ in self.variables]
+        vars_, chunks, ws, self.col_blocks = optim_tables(op, shapes, [o for o, _, _, _ in self.variables],
+                                                           [d for _, _, _, d in self.variables], self.opt)
+        mom_last = op == "apply_sm3" and self.opt.get("momentum", 0.0) > 0
+        for i, (_, _, slots, _) in enumerate(self.variables):
+            for k, s in enumerate(slots):
+                assert s.is_cuda and s.dtype == torch.float32 and s.is_contiguous()
+                vars_[i, 10 + (3 if mom_last and k == len(slots) - 1 else k)] = s.data_ptr()
+        self.nvars, self.nchunks = len(vars_), len(chunks)
+        self.vars_dev = torch.from_numpy(vars_).to(device)
+        self.chunks_dev = torch.from_numpy(chunks).to(device)
+        self.ws = torch.zeros(max(ws, 4), dtype=torch.float32, device=device)
+        o = self.opt
+        mom = o.get("momentum", 0.9 if op == "apply_momentum" else 0.0)
+        clip = o.get("clipping_threshold", 1.0)
+        self.hp = (ctypes.c_float * 12)(
+            o.get("beta1", 0.9) if op == "apply_lamb" else mom, o.get("beta2", 0.999), o.get("eps", 1e-6),
+            o.get("weight_decay", 0.0) or 0.0, o.get("eps1", 1e-30), o.get("eps2", 1e-3), -1.0 if clip is None else clip,
+            -1.0 if o.get("decay_rate") is None else o["decay_rate"], 1.0 if o.get("lr") is None else 0.0,
+            1.0 if o.get("multiply_by_parameter_scale", True) else 0.0, 1.0 if o.get("adapt_all", False) else 0.0,
+            1.0 if o.get("nesterov", False) else 0.0)
+
+
+def optim_step(plan: OptimPlan, master: torch.Tensor, grad: torch.Tensor, compute: Optional[torch.Tensor],
+               hyper: torch.Tensor) -> None:
+    """Apply `plan`'s update to every variable: fp32 master (and its bf16 compute copy) from the flat gradient buffer, with
+    the step's scalars read from the device tensor `hyper`.  CPU tensors: runtime/optimizers.py, one variable at a time."""
+    if not master.is_cuda:
+        from ..runtime.optimizers import STEP, Shards
+        for off, shape, slots, decay in plan.variables:
+            n = math.prod(shape)
+            STEP[plan.op](master[off:off + n].view(shape), grad[off:off + n].view(shape), slots, plan.opt, hyper, Shards(),
+                          decay=decay)
+            if compute is not None:
+                compute[off:off + n].copy_(master[off:off + n].to(compute.dtype))
+        return
+    _check(lib().tepd_optim_step(OPTIM_KINDS[plan.op], plan.vars_dev.data_ptr(), plan.chunks_dev.data_ptr(), plan.nvars,
+                                 plan.nchunks, plan.col_blocks, master.data_ptr(), grad.data_ptr(), _p(compute),
+                                 plan.ws.data_ptr(), hyper.data_ptr(), ctypes.addressof(plan.hp), _stream()), "optim_step")
+    _count(plan.launches)
 
 
 def cast_f32_bf16(src: torch.Tensor, dst: torch.Tensor) -> None:

@@ -307,6 +307,25 @@ class Executor:
         self._clip_scales: Dict[int, torch.Tensor] = {}
         self.pipeline_norm_divisor = 0       # set by a pipeline stage worker: SPMD replicas per stage (0 = not a pipeline)
         self.fused_apply_ok = self.clip is None and all(_whole(n) and n.op in FLAT_APPLY for n in self.apply_nodes)
+        # the optimizers with per-variable reductions (runtime/optimizers.py) run as one multi-tensor update over the flat
+        # buffers (ops.OptimPlan) when every apply node updates a whole, unsharded variable whose slots have the shapes the
+        # kernels expect; sharded views need reductions across ranks and keep the per-variable path
+        self.optim_plan: Optional[ops.OptimPlan] = None
+        if self.clip is None and self.apply_nodes and not self.fused_apply_ok:
+            op = self.apply_nodes[0].op
+            def _whole_var(n):
+                v = n.inputs[0]
+                if n.op != op or g.nodes[v.node].op != "parameter" or any(k > 1 for _, k, _ in self._shard_chain(v)):
+                    return False
+                want = ops.optim_slot_shapes(n.op, g.type_of(v).shape, self.opt)
+                return (want is not None and all(g.nodes[s.node].op == "state" for s in n.inputs[2:])
+                        and [tuple(g.type_of(s).shape) for s in n.inputs[2:]] == want)
+            if op in ops.OPTIM_KINDS and all(_whole_var(n) for n in self.apply_nodes):
+                st = self.store
+                self.optim_plan = ops.OptimPlan(op, self.opt, [
+                    (st.offset[n.inputs[0].node], st.shape[n.inputs[0].node], [st.state[s.node] for s in n.inputs[2:]],
+                     bool(n.attrs.get("decay", True))) for n in self.apply_nodes], self.device)
+                self.fused_apply_ok = True
         if not self.fused_apply_ok:
             self.grad_binding = {}  # general path: gradients flow through the environment, not the flat buffer
         self.update_target: Dict[Tuple[int, int], int] = {v.key(): var for var, v in g.updates.items()}
@@ -1079,6 +1098,8 @@ class Executor:
                            hyper=self.hyper)
         elif kind == "sgd":
             ops.sgd_step(st.master, st.grad, st.compute, self._lr(1e-2))
+        elif self.optim_plan is not None:
+            ops.optim_step(self.optim_plan, st.master, st.grad, st.compute, self.hyper)
 
     def _moe_choices(self, n: Node, gates: torch.Tensor) -> torch.Tensor:
         """Top-k expert choice of moe_dispatch_mask / moe_dispatch_mask_bwd node `n`: round r takes each token's r-th largest
