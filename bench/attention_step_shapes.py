@@ -4,9 +4,10 @@
 Per shape: the forward and backward call times (CUDA-event means over `--iters` calls after warm-up), then a torch.profiler
 pass in which each kernel of the calls (forward, delta, backward, dQ cast) gets its own time.  TFLOP/s counts
 4 * B * H * S^2 * D / 2 for the causal forward and 2.5 x that for the backward.  The card name, power limit and max SM clock
-are read (read-only nvidia-smi query) in the same run.
+are read (read-only nvidia-smi query) in the same run.  `--dropout P` also runs every shape with dropout P on the
+probabilities (the cost of generating the mask, forward and backward), alternating with the dropout-free calls.
 
-    python bench/attention_step_shapes.py [--iters 50] [--json out.json]
+    python bench/attention_step_shapes.py [--iters 50] [--dropout 0.1] [--json out.json]
 """
 from __future__ import annotations
 
@@ -27,9 +28,12 @@ from attention_heads import _card, _time_ms  # noqa: E402
 SHAPES = {"345M": (4, 16, 1024, 64), "1.3B": (2, 16, 2048, 128)}
 
 
-def run(name: str, iters: int) -> dict:
+def run(name: str, iters: int, pdrop: float = 0.0) -> dict:
     from tepdist_b200 import ops
     B, H, S, D = SHAPES[name]
+    drop = {}
+    if pdrop:
+        drop = {"pdrop": pdrop, "rng": ops.DropoutRng(1, torch.tensor([1, 0], device="cuda"), 1, global_shape=(B, S, H * D))}
     torch.manual_seed(0)
     qkv = torch.randn(B, S, H, 3, D, device="cuda", dtype=torch.bfloat16)
     q, k, v = qkv[:, :, :, 0], qkv[:, :, :, 1], qkv[:, :, :, 2]
@@ -37,12 +41,13 @@ def run(name: str, iters: int) -> dict:
     dqkv = torch.empty_like(qkv)
     fl = 4.0 * B * H * S * S * D * 0.5
     n0 = ops.launch_count()
-    o, lse = ops.attention_fwd(q, k, v, causal=True)
-    ops.attention_bwd(do, q, k, v, o, lse, causal=True, dqkv_out=dqkv)
+    o, lse = ops.attention_fwd(q, k, v, causal=True, **drop)
+    ops.attention_bwd(do, q, k, v, o, lse, causal=True, dqkv_out=dqkv, **drop)
     assert ops.launch_count() >= n0 + 4, "attention kernels did not run"
-    fwd = lambda: ops.attention_fwd(q, k, v, causal=True)  # noqa: E731
-    bwd = lambda: ops.attention_bwd(do, q, k, v, o, lse, causal=True, dqkv_out=dqkv)  # noqa: E731
-    r = {"shape": name, "B": B, "H": H, "S": S, "D": D, "fwd_ms": _time_ms(fwd, iters), "bwd_ms": _time_ms(bwd, iters)}
+    fwd = lambda: ops.attention_fwd(q, k, v, causal=True, **drop)  # noqa: E731
+    bwd = lambda: ops.attention_bwd(do, q, k, v, o, lse, causal=True, dqkv_out=dqkv, **drop)  # noqa: E731
+    r = {"shape": name, "B": B, "H": H, "S": S, "D": D, "pdrop": pdrop, "fwd_ms": _time_ms(fwd, iters),
+         "bwd_ms": _time_ms(bwd, iters)}
     r["fwd_tflops"] = fl / r["fwd_ms"] / 1e9
     r["bwd_tflops"] = 2.5 * fl / r["bwd_ms"] / 1e9
     torch.cuda.synchronize()
@@ -65,6 +70,7 @@ def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--json", default=None)
+    ap.add_argument("--dropout", type=float, default=0.0, help="also time every shape with this dropout on the probabilities")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("attention_step_shapes.py: no CUDA GPU; the timings are only meaningful on the H100")
@@ -73,10 +79,10 @@ def main() -> None:
     card = _card()
     print(f"# card: {card}  (name, power limit, max SM clock)")
     rows = []
-    for name in SHAPES:
-        r = run(name, a.iters)
+    for name, pdrop in [(n, p) for n in SHAPES for p in ((0.0, a.dropout) if a.dropout else (0.0,))]:
+        r = run(name, a.iters, pdrop)
         rows.append(r)
-        print(f"{name:5s} B {r['B']} H {r['H']} S {r['S']} D {r['D']} causal | fwd {r['fwd_ms']:.4f} ms {r['fwd_tflops']:6.1f} TFLOP/s"
+        print(f"{name:5s} B {r['B']} H {r['H']} S {r['S']} D {r['D']} causal p {pdrop:g} | fwd {r['fwd_ms']:.4f} ms {r['fwd_tflops']:6.1f} TFLOP/s"
               f" | bwd {r['bwd_ms']:.4f} ms {r['bwd_tflops']:6.1f} TFLOP/s", flush=True)
         for kname, ms in sorted(r["kernels_ms"].items(), key=lambda kv: -kv[1]):
             print(f"      {kname:32s} {ms:.4f} ms")

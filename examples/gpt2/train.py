@@ -4,6 +4,7 @@ random batch, like the reference's FAKE_INPUT server flag), `--data a.bin,b.bin`
 loader (tepdist_b200/data: memory-mapped uint16 / int32 token streams, windows of n_ctx + 1 tokens, stateless sampling), or
 `--data synthetic` for a fresh random batch every step from the same loader."""
 import argparse
+import dataclasses
 import os
 import sys
 import time
@@ -30,6 +31,9 @@ def main():
     ap.add_argument("--data", default=None, help="comma-separated token files (see tepdist_b200.data.write_token_file) or 'synthetic'")
     ap.add_argument("--data-int32", action="store_true", help="token files hold int32 ids (default uint16)")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--dropout", type=float, default=0.0,
+                    help="GPT-2's dropout: this probability on the embedding sum, the attention probabilities and every block output "
+                         "(embd_pdrop = attn_pdrop = resid_pdrop; the reference configuration uses 0.1)")
     ap.add_argument("--eot-token", type=int, default=None,
                     help="end-of-text token id (50256 for GPT-2): attention stays inside each packed document")
     ap.add_argument("--reset-position-ids", action="store_true",
@@ -37,6 +41,8 @@ def main():
     a = ap.parse_args()
     clip = {"clip_norm": a.clip_norm, "clip_norm_value": a.clip_norm_value} if a.clip_norm else {}
     cfg = CONFIGS[a.model]
+    if a.dropout:
+        cfg = dataclasses.replace(cfg, embd_pdrop=a.dropout, attn_pdrop=a.dropout, resid_pdrop=a.dropout)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     g = build_gpt2_graph(cfg, batch=a.batch * world, optimizer=a.optimizer, eot_token=a.eot_token,
                          reset_position_ids=a.reset_position_ids, **clip)

@@ -43,7 +43,7 @@ class CheckpointManager:
         tmp = prefix + ".tmp"
         os.makedirs(tmp, exist_ok=True)
         manifest: Dict[str, Any] = {"global_step": global_step, "rank": self.rank, "world": self.world, "vars": {},
-                                    "step_count": executor.step_count, "extra": extra or {}}
+                                    "step_count": executor.step_count, "drop_seed": executor.drop_seed, "extra": extra or {}}
         tensors: Dict[str, torch.Tensor] = {}
         # variables whose first / second moments live in the flat m / v buffers (others keep them as separate slot tensors)
         flat_moments = {pid for pid in st.order if st.moments_flat(pid)} if hasattr(st, "moments_flat") else set()
@@ -140,6 +140,7 @@ class CheckpointManager:
                 st.state[n.id].copy_(tensors[n.name].reshape(st.state[n.id].shape).to(st.device))
         st.sync_compute()
         executor.step_count = int(manifest.get("step_count", step))
+        executor.drop_seed = int(manifest.get("drop_seed", executor.drop_seed))   # a resumed run drops what the first would have
         return step
 
     # ------------------------------------------------------------------ restore into a DIFFERENT plan / world size
@@ -227,4 +228,5 @@ class CheckpointManager:
                 st.state[n.id].copy_(shard_of(full, n.attrs, executor.coords).reshape(st.state[n.id].shape).to(st.device))
         st.sync_compute()
         executor.step_count = int(writers[0][0].get("step_count", step))
+        executor.drop_seed = int(writers[0][0].get("drop_seed", executor.drop_seed))
         return step

@@ -206,21 +206,24 @@ void LayerNormBwdRule(Ctx& c) {
 double RingBytes(const TensorType& qkv, int num) { return (double)qkv.bytes() * (2.0 / 3.0) * (num - 1) / num; }
 // Document-masked attention (a 2nd input doc_start [B,S]; attention_bwd: a 5th) has no "seq" candidate: the ring does not carry
 // document starts, so context parallelism with document masks is not offered.  It splits over the batch (doc_start with it)
-// or over heads (doc_start replicated).
-void DocAttentionRule(Ctx& c, int qkv_idx) {
+// or over heads (doc_start replicated).  Attention with dropout uses the same two candidates, with or without doc_start.
+void NoRingAttentionRule(Ctx& c, int qkv_idx, bool has_doc) {
   const int64_t H = c.n.attr_i("heads");
   const int nin = c.nin();
   std::vector<DS> batch(nin, c.S(0)), heads(nin, c.S(2));
-  heads[nin - 1] = c.G();
+  if (has_doc) heads[nin - 1] = c.G();
   if (c.n.op == "attention_bwd") heads[3] = c.S(1);   // lse [B,H,S]
   if (c.divisible(c.in(qkv_idx), 0))
     c.add(batch, c.n.op == "attention" ? std::vector<DS>{c.S(0), c.S(0)} : std::vector<DS>{c.S(0)}, "batch");
   if (H % c.num == 0) c.add(heads, c.n.op == "attention" ? std::vector<DS>{c.S(2), c.S(1)} : std::vector<DS>{c.S(2)}, "heads");
   c.add_glue();
 }
+// Attention with dropout (attr pdrop > 0) has no "seq" candidate either: the ring's block kernels have no global query / key
+// offsets, so the mask of a split sequence would not be the one-device mask.
+bool HasAttnDropout(const Node& n) { return n.has("pdrop") && n.attr_f("pdrop") > 0.0; }
 void AttentionRule(Ctx& c, const RuleOptions& opt) {
   // qkv [B,S,H*3*D] (heads-major, so a plain last-dim split is a split over heads) -> o [B,S,H*D], lse [B,H,S]
-  if (c.nin() == 2) return DocAttentionRule(c, 0);
+  if (c.nin() == 2 || HasAttnDropout(c.n)) return NoRingAttentionRule(c, 0, c.nin() == 2);
   const int64_t H = c.n.attr_i("heads");
   const bool cp = opt.context_parallel && c.divisible(c.in(0), 1);   // "cp": the sequence split is the only way through attention
   if (c.divisible(c.in(0), 0) && !cp) c.add({c.S(0)}, {c.S(0), c.S(0)}, "batch");
@@ -229,7 +232,7 @@ void AttentionRule(Ctx& c, const RuleOptions& opt) {
   if (!cp) c.add_glue();   // (replicated attention = n x the S^2 FLOPs per rank: never what "cp" asks for)
 }
 void AttentionBwdRule(Ctx& c, const RuleOptions& opt) {
-  if (c.nin() == 5) return DocAttentionRule(c, 1);
+  if (c.nin() == 5 || HasAttnDropout(c.n)) return NoRingAttentionRule(c, 1, c.nin() == 5);
   const int64_t H = c.n.attr_i("heads");  // (do, qkv, o, lse) -> dqkv
   const bool cp = opt.context_parallel && c.divisible(c.in(1), 1);
   if (c.divisible(c.in(1), 0) && !cp) c.add({c.S(0), c.S(0), c.S(0), c.S(0)}, {c.S(0)}, "batch");
@@ -521,12 +524,13 @@ std::set<std::string>& UnknownOpsSeen() {
 std::vector<Candidate> EnumerateCandidates(const Graph& g, const Node& n, int num, const RuleOptions& opt) {
   Ctx c{g, n, num, {}};
   const std::string& op = n.op;
-  static const std::set<std::string> unary_linear = {"neg", "scale", "cast"};
+  // dropout / dropout_bwd multiply by a fixed mask: linear, the same mask on every partial sum
+  static const std::set<std::string> unary_linear = {"neg", "scale", "cast", "dropout", "dropout_bwd"};
   static const std::set<std::string> unary = {"gelu", "relu", "tanh", "exp", "log", "sqrt", "rsqrt", "sigmoid", "abs", "sign", "erf",
                                                "logical_not", "floor", "ceil", "silu"};
   static const std::set<std::string> binary_linear = {"add", "sub"};
   static const std::set<std::string> binary = {"mul", "div", "relu_bwd", "tanh_bwd", "gelu_bwd", "maximum", "minimum", "pow", "compare",
-                                                "logical_and", "logical_or", "sigmoid_bwd", "silu_bwd"};
+                                                "logical_and", "logical_or", "sigmoid_bwd", "silu_bwd", "dropout_add"};
   if (IsSource(op)) SourceRule(c);
   else if (unary_linear.count(op) || binary_linear.count(op)) Elementwise(c, true);
   else if (unary.count(op) || binary.count(op)) Elementwise(c, false);
@@ -722,7 +726,8 @@ std::vector<std::string> VerifyInfer(const Graph& g, int num) {
       }
       // shape algebra for elementwise families: out shard dim == max over operand shard dims (right-aligned broadcasting)
       static const std::set<std::string> ew = {"add", "sub", "mul", "div", "neg", "scale", "cast", "gelu", "relu", "tanh", "exp", "log",
-                                               "maximum", "minimum", "select", "clamp", "sqrt", "rsqrt", "sigmoid", "abs"};
+                                               "maximum", "minimum", "select", "clamp", "sqrt", "rsqrt", "sigmoid", "abs", "dropout",
+                                               "dropout_bwd", "dropout_add"};
       if (ew.count(n.op) && !c.outs.empty() && !c.outs[0].partial) {
         TensorType so = ShardType(n.outputs[0], c.outs[0]);
         for (size_t i = 0; i < c.ins.size(); ++i) {

@@ -3,6 +3,7 @@
 #include <cmath>
 #include <functional>
 #include <cstring>
+#include <stdexcept>
 
 namespace tepdist {
 
@@ -98,10 +99,13 @@ inline void PhiloxRound(uint32_t (&c)[4], uint32_t (&k)[2]) {
   k[0] += 0x9E3779B9u;
   k[1] += 0xBB67AE85u;
 }
-inline void PhiloxBlock(uint64_t seed, uint64_t block, uint32_t attempt, uint32_t (&out)[4]) {
-  uint32_t c[4] = {(uint32_t)block, (uint32_t)(block >> 32), attempt, 0u};
+inline void Philox10(uint64_t seed, uint32_t (&c)[4]) {
   uint32_t k[2] = {(uint32_t)seed, (uint32_t)(seed >> 32)};
   for (int i = 0; i < 10; ++i) PhiloxRound(c, k);
+}
+inline void PhiloxBlock(uint64_t seed, uint64_t block, uint32_t attempt, uint32_t (&out)[4]) {
+  uint32_t c[4] = {(uint32_t)block, (uint32_t)(block >> 32), attempt, 0u};
+  Philox10(seed, c);
   for (int i = 0; i < 4; ++i) out[i] = c[i];
 }
 inline float U01(uint32_t x) { return (float)((x >> 8) + 0.5f) * (1.0f / 16777216.0f); }  // (0,1)
@@ -145,6 +149,47 @@ std::vector<float> PhiloxFillShard(const std::string& kind, uint64_t seed, const
     PhiloxFill(kind, seed, run.first, run.second, mean, stddev, lo, hi, out.data() + o);
   }
   return out;
+}
+
+void DropoutKeep(uint64_t seed, uint32_t step, uint32_t site, int thr, bool attention, const std::vector<int64_t>& shape,
+                 const std::vector<int64_t>& start, const std::vector<int64_t>& len, uint8_t* out) {
+  const int r = (int)shape.size();
+  if (r == 0 || (int)start.size() != r || (int)len.size() != r || (attention && (r != 4 || shape[2] != shape[3])))
+    throw std::invalid_argument("DropoutKeep: the box must have the global shape's rank ([B, H, S, S] for attention)");
+  int64_t n = 1;
+  for (int d = 0; d < r; ++d) {
+    if (start[d] < 0 || len[d] < 0 || start[d] + len[d] > shape[d]) throw std::invalid_argument("DropoutKeep: box outside the shape");
+    n *= len[d];
+  }
+  std::vector<int64_t> idx(start);   // global coordinates of the current element (row-major walk over the box)
+  uint32_t c[4], last0 = 0, last1 = 0;
+  bool have = false;
+  for (int64_t e = 0; e < n; ++e) {
+    uint32_t c0, c1, byte;
+    if (attention) {
+      const int64_t S = shape[2], q = idx[2], k = idx[3];
+      c0 = (uint32_t)(((k >> 5) << 2) | ((k >> 1) & 3));
+      c1 = (uint32_t)((idx[0] * shape[1] + idx[1]) * S + (q & ~int64_t(8)));
+      byte = (uint32_t)(8 * ((q >> 3) & 1) + 2 * ((k >> 3) & 3) + (k & 1));
+    } else {
+      int64_t row = 0;
+      for (int d = 0; d < r - 1; ++d) row = row * shape[d] + idx[d];
+      const int64_t col = idx[r - 1];
+      c0 = (uint32_t)(col >> 4);
+      c1 = (uint32_t)row;
+      byte = (uint32_t)(col & 15);
+    }
+    if (!have || c0 != last0 || c1 != last1) {
+      c[0] = c0; c[1] = c1; c[2] = step; c[3] = site;
+      Philox10(seed, c);
+      last0 = c0; last1 = c1; have = true;
+    }
+    out[e] = ((c[byte >> 2] >> (8 * (byte & 3))) & 0xffu) >= (uint32_t)thr;
+    for (int d = r - 1; d >= 0; --d) {
+      if (++idx[d] < start[d] + len[d]) break;
+      idx[d] = start[d];
+    }
+  }
 }
 
 }  // namespace tepdist

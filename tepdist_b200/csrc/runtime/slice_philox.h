@@ -31,4 +31,13 @@ std::vector<float> PhiloxFillShard(const std::string& kind, uint64_t seed, const
                                    const std::vector<DimStrategy>& levels, const std::vector<int>& ids, float mean, float stddev,
                                    float lo, float hi);
 
+// Dropout keep mask (DESIGN.md "Dropout"): out[e] = 1 iff element e of the box [start, start + len) of a tensor of GLOBAL
+// shape `shape` is kept.  Philox4x32-10 keyed by `seed`, counter (column group, row, step, site); an element is kept iff its
+// byte of the call's 16 is >= thr.  Elementwise: row = the flattened leading coordinates, 16 consecutive columns per call.
+// attention (shape [B, H, S, S], (b, h, query, key)): one call per (b, h, 16-query block, 32-key block, query % 8,
+// (key % 8) / 2), the 16 elements a thread of the forward kernel holds in its score fragment.  The CUDA kernels
+// (ops/csrc/dropout_philox.cuh) produce the same bits.
+void DropoutKeep(uint64_t seed, uint32_t step, uint32_t site, int thr, bool attention, const std::vector<int64_t>& shape,
+                 const std::vector<int64_t>& start, const std::vector<int64_t>& len, uint8_t* out);
+
 }  // namespace tepdist

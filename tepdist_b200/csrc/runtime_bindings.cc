@@ -129,6 +129,13 @@ void BindRuntime(py::module_& m) {
     out.resize(ShardShape(shape, levels));
     return out;
   });
+  m.def("dropout_keep", [](uint64_t seed, uint32_t step, uint32_t site, int thr, const std::vector<int64_t>& shape,
+                           const std::vector<int64_t>& start, const std::vector<int64_t>& len, bool attention) {
+    py::array_t<uint8_t> out(len);
+    DropoutKeep(seed, step, site, thr, attention, shape, start, len, out.mutable_data());
+    return out;
+  }, py::arg("seed"), py::arg("step"), py::arg("site"), py::arg("thr"), py::arg("shape"), py::arg("start"), py::arg("len"),
+     py::arg("attention") = false);
 
   // ---- ServiceEnv
   py::class_<ServiceEnv>(m, "ServiceEnv")

@@ -108,6 +108,20 @@ struct Rewriter {
         a["cp_nums"] = nm;
       }
     }
+    const bool dropout = op == "dropout" || op == "dropout_bwd" || op == "dropout_add" ||
+                         ((op == "attention" || op == "attention_bwd") && n.has("pdrop") && n.attr_f("pdrop") > 0.0);
+    if (dropout) {
+      // a dropout mask is defined on GLOBAL coordinates: remember the unsharded output shape and how every level cut it, so
+      // the runtime can turn its mesh coordinates into the shard's offsets (runtime/executor.py Executor._drop_rng)
+      if (!n.has("drop_full")) a["drop_full"] = n.outputs[0].dims;
+      if (c.outs[0].is_split()) {
+        std::vector<int64_t> dims = n.attr_v("drop_dims"), nums = n.attr_v("drop_nums"), lvls = n.attr_v("drop_levels");
+        dims.push_back(c.outs[0].dim);
+        nums.push_back(num);
+        lvls.push_back(level);
+        a["drop_dims"] = dims; a["drop_nums"] = nums; a["drop_levels"] = lvls;
+      }
+    }
     if (op == "softmax_xent") {
       const TensorType& l = g.type(n.inputs[0]);
       int64_t tokens = n.has("global_tokens") ? n.attr_i("global_tokens") : l.numel() / l.dims.back();

@@ -18,6 +18,12 @@ class GraphBuilder:
         self.g = Graph(name)
         self.cd = compute_dtype
         self._scope: List[str] = []
+        self._sites = 0
+
+    def _site(self) -> int:
+        """A new dropout site id (1, 2, ...): one of the inputs of the mask definition (DESIGN.md "Dropout")."""
+        self._sites += 1
+        return self._sites
 
     # ------------------------------------------------------------------ helpers
     def _n(self, op, inputs, outs, attrs=None, name="", group=None) -> Node:
@@ -89,17 +95,45 @@ class GraphBuilder:
     def gelu(self, x: Value, name="gelu") -> Value:
         return self._n("gelu", [x], [self.t(x)], {}, name).out()
 
+    @staticmethod
+    def _check_p(p: float, what: str) -> float:
+        p = float(p)
+        if not 0.0 <= p < 1.0:
+            raise ValueError(f"{what}: dropout probability {p} outside [0, 1)")
+        return p
+
+    def dropout(self, x: Value, p: float, name="dropout") -> Value:
+        """Training-mode dropout: x * Z, Z = 0 with probability p (quantised to 1/256) and 1 / (1 - p) otherwise; the mask is
+        a function of (seed, step, this site, global coordinates) only (DESIGN.md "Dropout").  p = 0 adds no node.  On the
+        GPU, x must be bf16 with a last dim (per shard) that is a multiple of 16 (dropout_kernel's 16-element vectors); an
+        Executor on a CUDA device refuses other dropout nodes when it is built."""
+        if self._check_p(p, "dropout") == 0.0:
+            return x
+        return self._n("dropout", [x], [self.t(x)], {"p": float(p), "site": self._site()}, name).out()
+
+    def dropout_add(self, x: Value, residual: Value, p: float, name="dropout_add") -> Value:
+        """residual + dropout(x, p) in one op (a block's output joining the residual stream); p = 0 is a plain add."""
+        if self._check_p(p, "dropout_add") == 0.0:
+            return self.add(x, residual, name=name)
+        if tuple(self.t(x).shape) != tuple(self.t(residual).shape):
+            raise ValueError(f"dropout_add: x {self.t(x).shape} and residual {self.t(residual).shape} differ")
+        return self._n("dropout_add", [x, residual], [self.t(x)], {"p": float(p), "site": self._site()}, name).out()
+
     def attention(self, qkv: Value, heads: int, causal: bool = True, doc_starts: Optional[Value] = None,
-                  name="attn") -> Value:
+                  pdrop: float = 0.0, name="attn") -> Value:
         """Fused attention over qkv [B, S, 3C] (heads-major).  `doc_starts` (causal only) restricts every query to the keys
-        of its own document."""
+        of its own document.  `pdrop`: dropout on the attention probabilities (as `dropout`; the softmax statistics stay
+        those of the undropped probabilities)."""
         B, S, C3 = self.t(qkv).shape
         C = C3 // 3
         if doc_starts is not None and not causal:
             raise ValueError("attention: document masking (doc_starts) is defined for causal attention only")
+        attrs = {"heads": heads, "causal": causal}
+        if self._check_p(pdrop, "attention") > 0.0:
+            attrs.update(pdrop=float(pdrop), site=self._site())
         ins = [qkv] + ([doc_starts] if doc_starts is not None else [])
         n = self._n("attention", ins, [TensorType((B, S, C), self.t(qkv).dtype), TensorType((B, heads, S), "f32")],
-                    {"heads": heads, "causal": causal}, name)
+                    attrs, name)
         return n.out(0)
 
     def softmax_xent(self, logits: Value, labels: Value, vocab: Optional[int] = None, name="loss") -> Value:
@@ -355,6 +389,10 @@ def backward(b: GraphBuilder, loss: Value) -> Dict[int, Value]:
             push(x, nb.out(0)); push(gm, nb.out(1)); push(bt, nb.out(2))
         elif n.op == "gelu":
             push(n.inputs[0], B("gelu_bwd", [dy, n.inputs[0]], [T(n.inputs[0])], {}, grp).out())
+        elif n.op in ("dropout", "dropout_add"):    # the same mask (same site) applied to the gradient
+            push(n.inputs[0], B("dropout_bwd", [dy], [T(n.inputs[0])], {"p": n.attrs["p"], "site": n.attrs["site"]}, grp).out())
+            if n.op == "dropout_add":
+                push(n.inputs[1], dy)
         elif n.op == "attention":
             qkv = n.inputs[0]
             push(qkv, B("attention_bwd", [dy, qkv, Value(n.id, 0), Value(n.id, 1)] + n.inputs[1:], [T(qkv)], dict(n.attrs),

@@ -1,6 +1,7 @@
 """GPT-2 (the reference's headline example, examples/GPT2/models/gpt2/gpt2.py + *.json) expressed in
 planner IR.  Structure follows SURVEY Appendix C: pre-LN blocks, tanh-GELU MLP (4x), separate untied LM
-head, learned positions, no dropout (the reference's dropout is a no-op), AdamW; Q/K/V projections are
+head, learned positions, optional dropout (`embd_pdrop` on the embedding sum, `attn_pdrop` on the attention probabilities,
+`resid_pdrop` on each block output before its residual add; 0 by default), AdamW; Q/K/V projections are
 fused into one [3C, C] matmul (same math as the reference's three conv1d's).  The vocabulary is padded to
 a multiple of 128 for the tensor-core tile; padded logits are masked inside the fused loss kernel.
 """
@@ -24,6 +25,9 @@ class GPT2Config:
     lr: float = 1e-4
     weight_decay: float = 0.01
     name: str = "gpt2-345M"
+    embd_pdrop: float = 0.0
+    attn_pdrop: float = 0.0
+    resid_pdrop: float = 0.0
 
     @property
     def padded_vocab(self) -> int:
@@ -73,22 +77,29 @@ def build_gpt2_graph(cfg: GPT2Config, batch: int | None = None, optimizer: str =
         wpe = b.parameter("wpe", (S, C), nrm(0.01))
         ds = b.doc_starts(tokens, eot_token) if eot_token is not None else None
         x = b.embedding(tokens, wte, wpe, doc_starts=ds if reset_position_ids else None)
+        x = b.dropout(x, cfg.embd_pdrop, name="embd_drop")
+        # with resid_pdrop the projections end at their bias and dropout_add joins the residual stream (so a tensor-parallel
+        # plan runs their unfused GEMM + all-reduce form: the fused GEMM + all-reduce chain ends in a plain residual add)
+        def proj(h_, w_, b_, res_, name_):
+            if cfg.resid_pdrop:
+                return b.dropout_add(b.linear(h_, w_, b_, name=name_), res_, cfg.resid_pdrop, name=name_ + "/drop")
+            return b.linear(h_, w_, b_, residual=res_, name=name_)
         for l in range(cfg.n_layer):
             with b.scope(f"h{l}"):
                 g1 = b.parameter("ln_1/g", (C,), const(1.0)); b1 = b.parameter("ln_1/b", (C,), const(0.0))
                 h = b.layernorm(x, g1, b1, name="ln_1")
                 w_qkv = b.parameter("attn/c_attn/w", (3 * C, C), nrm(0.02)); b_qkv = b.parameter("attn/c_attn/b", (3 * C,), const(0.0))
                 qkv = b.linear(h, w_qkv, b_qkv, name="attn/c_attn")
-                a = b.attention(qkv, heads=H, causal=True, doc_starts=ds, name="attn/core")
+                a = b.attention(qkv, heads=H, causal=True, doc_starts=ds, pdrop=cfg.attn_pdrop, name="attn/core")
                 w_o = b.parameter("attn/c_proj/w", (C, C), nrm(0.02 / math.sqrt(2 * cfg.n_layer))); b_o = b.parameter("attn/c_proj/b", (C,), const(0.0))
-                x = b.linear(a, w_o, b_o, residual=x, name="attn/c_proj")
+                x = proj(a, w_o, b_o, x, "attn/c_proj")
                 g2 = b.parameter("ln_2/g", (C,), const(1.0)); b2 = b.parameter("ln_2/b", (C,), const(0.0))
                 h = b.layernorm(x, g2, b2, name="ln_2")
                 w_fc = b.parameter("mlp/c_fc/w", (4 * C, C), nrm(0.02)); b_fc = b.parameter("mlp/c_fc/b", (4 * C,), const(0.0))
                 f = b.linear(h, w_fc, b_fc, name="mlp/c_fc")
                 f = b.gelu(f, name="mlp/gelu")
                 w_p = b.parameter("mlp/c_proj/w", (C, 4 * C), nrm(0.02 / math.sqrt(2 * cfg.n_layer))); b_p = b.parameter("mlp/c_proj/b", (C,), const(0.0))
-                x = b.linear(f, w_p, b_p, residual=x, name="mlp/c_proj")
+                x = proj(f, w_p, b_p, x, "mlp/c_proj")
         gf = b.parameter("ln_f/g", (C,), const(1.0)); bf = b.parameter("ln_f/b", (C,), const(0.0))
         h = b.layernorm(x, gf, bf, name="ln_f")
         w_out = b.parameter("output", (Vp, C), nrm(0.02))
@@ -98,4 +109,6 @@ def build_gpt2_graph(cfg: GPT2Config, batch: int | None = None, optimizer: str =
                                                      **opt_hp})      # (opt_hp: clip_norm / clip_norm_value / schedule / ...)
     g.meta["model"] = {"family": "gpt2", "name": cfg.name, "n_layer": cfg.n_layer, "n_embd": C, "n_head": H,
                        "n_ctx": S, "n_vocab": V, "batch": B, "eot_token": eot_token, "reset_position_ids": bool(reset_position_ids)}
+    if cfg.embd_pdrop or cfg.attn_pdrop or cfg.resid_pdrop:
+        g.meta["model"].update(embd_pdrop=cfg.embd_pdrop, attn_pdrop=cfg.attn_pdrop, resid_pdrop=cfg.resid_pdrop)
     return g

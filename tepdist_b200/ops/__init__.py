@@ -10,6 +10,7 @@ from __future__ import annotations
 import ctypes
 import math
 import os
+from dataclasses import dataclass
 from typing import Optional
 
 import torch
@@ -71,7 +72,7 @@ def _count(n: int = 1) -> None:
     _launches += n
 
 
-_vp, _i, _ll, _f = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float
+_vp, _i, _ll, _f, _ull = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float, ctypes.c_ulonglong
 
 
 class _Sig:
@@ -108,9 +109,11 @@ class _Sig:
     tepd_gap_bwd_nhwc = [_vp, _vp, _i, _i, _i, _vp]
     tepd_attn_merge = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]
     tepd_attn_ring_accum = [_vp, _vp, _vp, _ll, _i, _i, _vp]
-    tepd_attn_fwd = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _ll, _ll, _ll, _vp, _vp]
+    tepd_attn_fwd = [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _ll, _ll, _ll, _vp, _vp,
+                     _ull, _vp, _ll, _ll, _i, _i, _i, _i, _i]
     tepd_attn_bwd = [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i,
-                     _ll, _ll, _ll, _ll, _ll, _ll, _vp, _vp]
+                     _ll, _ll, _ll, _ll, _ll, _ll, _vp, _vp, _ull, _vp, _ll, _ll, _i, _i, _i, _i, _i, _vp]
+    tepd_dropout = [_vp, _vp, _vp, _ll, _i, _i, _ll, _ll, _ll, _ll, _ll, _ull, _vp, _i, _i, _f, _vp]
 
 
 def _stream() -> int:
@@ -952,6 +955,103 @@ def cast_f32_bf16(src: torch.Tensor, dst: torch.Tensor) -> None:
         return
     _check(lib().tepd_cast_f32_bf16(src.data_ptr(), dst.data_ptr(), src.numel(), _stream()), "cast_f32_bf16")
     _count()
+
+
+# --------------------------------------------------------------------------------------------- dropout
+def dropout_threshold(p: float) -> int:
+    """The keep threshold byte of drop probability p: an element is dropped iff its mask byte is < round(256 p), so p is
+    quantised to 1/256 (p = 0.1 drops 26/256 of the elements).  p must lie in [0, 1)."""
+    p = float(p)
+    if not 0.0 <= p < 1.0:
+        raise ValueError(f"dropout probability {p}: expected 0 <= p < 1")
+    return min(255, int(round(p * 256)))
+
+
+@dataclass
+class DropoutRng:
+    """Where one dropout site's mask comes from (DESIGN.md "Dropout").  Every mask element is a function of (seed, step,
+    site, the element's coordinates in the GLOBAL tensor) only, so a shard passes where it sits in the global tensor:
+      state         int64 [2] on the data's device: (optimizer step, pipeline micro-batch index) -- read by the kernels
+                    from device memory, so a captured CUDA graph uses the values of the step it replays
+      offsets       per dim of the op's output: the shard's global start (excluding the micro-batch term)
+      micro         per dim: how far one micro-batch index moves that start (0 = not split into micro-batches)
+      global_shape  per dim: the global extent (for attention, of its [B, S, C] output; C counts heads x head width)"""
+    seed: int
+    state: torch.Tensor
+    site: int
+    offsets: tuple = ()
+    micro: tuple = ()
+    global_shape: tuple = ()
+
+    def starts(self, ndim: int) -> list:
+        """Global start of the shard per dim, micro-batch term included (host: reads `state`)."""
+        m = int(self.state[1]) if any(self.micro) else 0
+        off = list(self.offsets) or [0] * ndim
+        mic = list(self.micro) or [0] * ndim
+        return [o + m * k for o, k in zip(off, mic)]
+
+
+def _ew_layout(shape, rng: DropoutRng):
+    """[d0, .., dn-1] -> the kernel's [A, R, C] with global row (a_off + m a_micro + a) Rg + r_off + r: A = d0, R = the
+    product of the middle dims, which may be cut on the first of them only."""
+    shape = tuple(shape)
+    n = len(shape)
+    gs = tuple(rng.global_shape) or shape
+    off = tuple(rng.offsets) or (0,) * n
+    mic = tuple(rng.micro) or (0,) * n
+    if n < 2:
+        raise ValueError(f"dropout: rank {n} tensor; expected [rows.., columns]")
+    for d in range(2, n - 1):
+        if shape[d] != gs[d] or off[d] or mic[d]:
+            raise ValueError(f"dropout: dim {d} of a {shape} shard of {gs} is cut; only the first two dims and the last may be")
+    if any(mic[1:]):
+        raise ValueError("dropout: micro-batches must split dim 0")
+    inner = math.prod(gs[2:-1]) if n > 3 else 1
+    A, R, C = shape[0], math.prod(shape[1:-1]), shape[-1]
+    Rg = gs[1] * inner if n > 2 else 1
+    r_off = off[1] * inner if n > 2 else 0
+    return A, R, C, off[0], mic[0], r_off, Rg, off[-1], gs
+
+
+def _host_keep(rng: DropoutRng, thr: int, shape) -> torch.Tensor:
+    """The host reference mask (bool, `shape`) of this elementwise shard: _C.dropout_keep, the one implementation outside
+    CUDA."""
+    from .. import _C
+    k = _C.dropout_keep(rng.seed, int(rng.state[0]), rng.site, thr, list(rng.global_shape) or list(shape),
+                        rng.starts(len(shape)), list(shape), False)
+    return torch.from_numpy(k).bool()
+
+
+def dropout(x: torch.Tensor, p: float, rng: DropoutRng, res: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """y = x * Z (+ res): Z = the scaled keep mask of (rng, p), 256 / (256 - thr) where kept and 0 where dropped.  Also the
+    backward of a dropout (dy * Z, the same site) and, with `res`, dropout followed by the residual add."""
+    thr = dropout_threshold(p)
+    scale = 256.0 / (256 - thr)
+    if not x.is_cuda:
+        keep = _host_keep(rng, thr, tuple(x.shape)).to(x.device)
+        y = torch.where(keep, x.float() * scale, torch.zeros((), dtype=torch.float32))
+        if res is not None:
+            y = y + res.float()
+        return y.to(x.dtype)
+    A, R, C, a_off, a_micro, r_off, Rg, c_off, _ = _ew_layout(x.shape, rng)
+    if x.dtype != torch.bfloat16 or C % 16 or c_off % 16 or (res is not None and (res.dtype != x.dtype or res.shape != x.shape)):
+        raise ValueError(f"dropout kernel: bf16 [.., C] with C % 16 == 0 and a column offset % 16 == 0 (and a residual of the same "
+                         f"shape); got {x.dtype} {tuple(x.shape)} at column {c_off}"
+                         + ("" if res is None else f", residual {res.dtype} {tuple(res.shape)}"))
+    if rng.state.device != x.device or rng.state.dtype != torch.int64:
+        raise ValueError("dropout: rng.state must be an int64 tensor on the data's device")
+    xc = x.contiguous()
+    rc = None if res is None else res.contiguous()
+    y = torch.empty_like(xc)
+    _check(lib().tepd_dropout(xc.data_ptr(), _p(rc), y.data_ptr(), A, R, C, a_off, a_micro, r_off, Rg, c_off, rng.seed,
+                              rng.state.data_ptr(), rng.site, thr, scale, _stream()), "dropout")
+    _count()
+    return y
+
+
+def dropout_add(x: torch.Tensor, res: torch.Tensor, p: float, rng: DropoutRng) -> torch.Tensor:
+    """res + dropout(x): one pass."""
+    return dropout(x, p, rng, res)
 
 
 # --------------------------------------------------------------------------------------------- attention

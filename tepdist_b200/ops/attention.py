@@ -10,6 +10,10 @@ plain torch math, which materialises [B, H, S, S] fp32 scores, and warn once per
 
 Document masking (packed rows): with ``doc_start`` (int32 [B, S], non-decreasing along S, see ``ops.doc_starts``) query s
 attends to keys doc_start[b, s] <= k <= s.  It is defined for causal attention only.
+
+Dropout on the probabilities (``pdrop`` > 0 with ``rng``, an ``ops.DropoutRng`` describing the [B, S, H * D] output): the
+softmax statistics (``lse``) come from the undropped probabilities and O = (P Z) V, Z the scaled keep mask of DESIGN.md
+"Dropout" at the GLOBAL (batch, head, query, key) of each element -- padded shapes keep the mask of their real pairs.
 """
 from __future__ import annotations
 
@@ -70,7 +74,57 @@ def _warn_torch_math(S: int, D: int, causal: bool) -> None:
                f"[B, H, {S}, {S}] fp32 scores")
 
 
-def _ref_fwd(q, k, v, scale, causal, doc_start=None):
+def keep_mask(rng, pdrop: float, B: int, H: int, S: int, D: int) -> torch.Tensor:
+    """Host reference of the attention dropout mask of this shard: bool [B, H, S (query), S (key)] (_C.dropout_keep)."""
+    from .. import _C
+    from . import dropout_threshold
+    Bg, Sg, Cg = tuple(rng.global_shape) or (B, S, H * D)
+    b0, s0, c0 = rng.starts(3)
+    if s0 != 0 or Sg != S:
+        raise ValueError("attention dropout: the sequence must not be split (context parallelism has no global key offsets)")
+    k = _C.dropout_keep(rng.seed, int(rng.state[0]), rng.site, dropout_threshold(pdrop), [Bg, Cg // D, S, S], [b0, c0 // D, 0, 0],
+                        [B, H, S, S], True)
+    return torch.from_numpy(k).bool()
+
+
+def _drop_scale(pdrop: float) -> float:
+    from . import dropout_threshold
+    return 256.0 / (256 - dropout_threshold(pdrop))
+
+
+def _drop_args(pdrop: float, rng, B: int, H: int, S: int, D: int) -> tuple:
+    """The kernels' dropout arguments (seed, state, b_off, b_micro, h_off, H_glob, S_real, site, thr); no dropout: rng = 0."""
+    if not pdrop:
+        return (0, None, 0, 0, 0, 0, 0, 0, 0)
+    from . import dropout_threshold
+    if rng is None:
+        raise ValueError("attention: pdrop > 0 needs rng (an ops.DropoutRng)")
+    thr = dropout_threshold(pdrop)
+    Bg, Sg, Cg = tuple(rng.global_shape) or (B, S, H * D)
+    off = tuple(rng.offsets) or (0, 0, 0)
+    mic = tuple(rng.micro) or (0, 0, 0)
+    if off[1] or mic[1] or mic[2] or Sg != S or off[2] % D or Cg % D:
+        raise ValueError(f"attention dropout: shard offsets {off} / micro {mic} of global {(Bg, Sg, Cg)}: the sequence must not be "
+                         "split and heads must be whole")
+    if rng.state.device.type != "cuda" or rng.state.dtype != torch.int64:
+        raise ValueError("attention dropout: rng.state must be an int64 CUDA tensor")
+    return (rng.seed, rng.state.data_ptr(), off[0], mic[0], off[2] // D, Cg // D, S, rng.site, thr)
+
+
+_ZERO_DOCS: dict = {}
+
+
+def _zero_docs(B: int, S: int, device) -> torch.Tensor:
+    """int32 zeros [B * S]: the document starts the D = 128 dropout backward reads when there are no documents (it always runs
+    its document-mask instantiation, see tepd_attn_bwd).  Kept for the life of the process, one per device and size, so a CUDA
+    graph that captured a backward never reads freed memory."""
+    key = (str(device), B * S)
+    if key not in _ZERO_DOCS:
+        _ZERO_DOCS[key] = torch.zeros(B * S, dtype=torch.int32, device=device)
+    return _ZERO_DOCS[key]
+
+
+def _ref_fwd(q, k, v, scale, causal, doc_start=None, pdrop: float = 0.0, rng=None):
     # q,k,v: [B,S,H,D] -> fp32 math in [B,H,S,D]
     qf, kf, vf = (t.float().permute(0, 2, 1, 3) for t in (q, k, v))
     s = torch.matmul(qf, kf.transpose(-1, -2)) * scale
@@ -79,28 +133,35 @@ def _ref_fwd(q, k, v, scale, causal, doc_start=None):
         s = s.masked_fill(~mask, float("-inf"))
     lse = torch.logsumexp(s, -1)  # [B,H,S]
     p = torch.exp(s - lse.unsqueeze(-1))
-    o = torch.matmul(p, vf).permute(0, 2, 1, 3).contiguous()
+    pz = p
+    if pdrop:
+        B, S, H, D = q.shape
+        pz = p * keep_mask(rng, pdrop, B, H, S, D).to(p.device) * _drop_scale(pdrop)
+    o = torch.matmul(pz, vf).permute(0, 2, 1, 3).contiguous()
     return o.to(q.dtype), lse, p
 
 
 def attention_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: float | None = None,
-                  causal: bool = True, doc_start: torch.Tensor | None = None):
-    """Returns (o [B,S,H,D], lse [B,H,S]).  ``doc_start`` (int32 [B, S]) adds the document mask."""
+                  causal: bool = True, doc_start: torch.Tensor | None = None, pdrop: float = 0.0, rng=None, _drop=None):
+    """Returns (o [B,S,H,D], lse [B,H,S]).  ``doc_start`` (int32 [B, S]) adds the document mask; ``pdrop`` / ``rng`` dropout
+    on the probabilities (module docstring)."""
     B, S, H, D = q.shape
     _check_doc(doc_start, causal)
     if scale is None:
         scale = 1.0 / math.sqrt(D)
     if not q.is_cuda:
-        o, lse, _ = _ref_fwd(q, k, v, scale, causal, doc_start)
+        o, lse, _ = _ref_fwd(q, k, v, scale, causal, doc_start, pdrop, rng)
         return o, lse
+    if _drop is None:
+        _drop = _drop_args(pdrop, rng, B, H, S, D)
     if D not in _KERNEL_WIDTHS or S % 128:
         if _can_pad(S, D, causal):
             W = _kernel_width(D)
             qp, kp, vp = (_pad_sd(t, S, D, W) for t in (q, k, v))
-            o, lse = attention_fwd(qp, kp, vp, scale, causal, _pad_doc(doc_start, S))
+            o, lse = attention_fwd(qp, kp, vp, scale, causal, _pad_doc(doc_start, S), _drop=_drop)
             return o[:, :S, :, :D].contiguous(), lse[:, :, :S].contiguous()
         _warn_torch_math(S, D, causal)
-        o, lse, _ = _ref_fwd(q, k, v, scale, causal, doc_start)   # shapes the wgmma kernels do not cover: plain torch math
+        o, lse, _ = _ref_fwd(q, k, v, scale, causal, doc_start, pdrop, rng)   # shapes the wgmma kernels do not cover: torch math
         return o, lse
     from . import lib, _check, _count, _stream, _doc_ptr, _p
     assert q.dtype == torch.bfloat16 and q.stride(3) == 1
@@ -109,16 +170,20 @@ def attention_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: floa
     o = torch.empty(B, S, H, D, dtype=q.dtype, device=q.device)
     lse = torch.empty(B, H, S, dtype=torch.float32, device=q.device)
     _check(lib().tepd_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), B, H, S, D,
-                               float(scale), int(causal), q.stride(0), q.stride(1), q.stride(2), _stream(), _p(ds)),
+                               float(scale), int(causal), q.stride(0), q.stride(1), q.stride(2), _stream(), _p(ds), *_drop),
            "attn_fwd")
     _count()
     return o, lse
 
 
 def attention_bwd(do: torch.Tensor, q, k, v, o, lse, scale: float | None = None, causal: bool = True,
-                  dqkv_out: torch.Tensor | None = None, doc_start: torch.Tensor | None = None):
-    """Returns (dq, dk, dv) as [B,S,H,D] views (of ``dqkv_out`` [B,S,H,3,D] when given)."""
+                  dqkv_out: torch.Tensor | None = None, doc_start: torch.Tensor | None = None, pdrop: float = 0.0, rng=None,
+                  _drop=None):
+    """Returns (dq, dk, dv) as [B,S,H,D] views (of ``dqkv_out`` [B,S,H,3,D] when given).  With dropout (the forward's pdrop
+    and rng): dV = (P Z)^T dO, dS = P (dP Z - delta)."""
     B, S, H, D = q.shape
+    if q.is_cuda and _drop is None:
+        _drop = _drop_args(pdrop, rng, B, H, S, D)
     _check_doc(doc_start, causal)
     if scale is None:
         scale = 1.0 / math.sqrt(D)
@@ -130,7 +195,7 @@ def attention_bwd(do: torch.Tensor, q, k, v, o, lse, scale: float | None = None,
         W = _kernel_width(D)
         lse_p = lse if Sp == S else torch.nn.functional.pad(lse, (0, Sp - S))
         gq, gk, gv = attention_bwd(*(_pad_sd(t, S, D, W) for t in (do, q, k, v, o)), lse_p, scale, causal,
-                                   doc_start=_pad_doc(doc_start, S))
+                                   doc_start=_pad_doc(doc_start, S), _drop=_drop)
         dq.copy_(gq[:, :S, :, :D]); dk.copy_(gk[:, :S, :, :D]); dv.copy_(gv[:, :S, :, :D])
         return dq, dk, dv
     if not q.is_cuda or D not in _KERNEL_WIDTHS or S % 128:
@@ -145,8 +210,11 @@ def attention_bwd(do: torch.Tensor, q, k, v, o, lse, scale: float | None = None,
         if mask is not None:
             sc = sc.masked_fill(~mask, float("-inf"))
         p = torch.exp(sc - lse.float().unsqueeze(-1))
-        dvf = torch.matmul(p.transpose(-1, -2), dof)
+        z = keep_mask(rng, pdrop, B, H, S, D).to(p.device) * _drop_scale(pdrop) if pdrop else None
+        dvf = torch.matmul((p if z is None else p * z).transpose(-1, -2), dof)
         dp = torch.matmul(dof, vf.transpose(-1, -2))
+        if z is not None:
+            dp = dp * z
         delta = (dof * o.float().permute(0, 2, 1, 3)).sum(-1, keepdim=True)
         ds = p * (dp - delta) * scale
         dqf = torch.matmul(ds, kf)
@@ -159,11 +227,12 @@ def attention_bwd(do: torch.Tensor, q, k, v, o, lse, scale: float | None = None,
     do = do.contiguous()
     assert o.is_contiguous() and do.is_contiguous()
     ds = _doc_ptr(doc_start, B, S)
+    zd = _zero_docs(B, S, q.device) if _drop[1] is not None and D == 128 and ds is None else None
     # dq accumulator: persistent self-clearing fp32 workspace inside the library (no per-call memset)
     _check(lib().tepd_attn_bwd(do.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
                                None, dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, H, S, D,
                                float(scale), int(causal), q.stride(0), q.stride(1), q.stride(2),
-                               dq.stride(0), dq.stride(1), dq.stride(2), _stream(), _p(ds)), "attn_bwd")
+                               dq.stride(0), dq.stride(1), dq.stride(2), _stream(), _p(ds), *_drop, _p(zd)), "attn_bwd")
     _count(3)
     return dq, dk, dv
 

@@ -13,6 +13,7 @@
 // this kernel is the H100-native replacement.
 #include "sm90_ptx.cuh"
 #include "launch.cuh"
+#include "dropout_philox.cuh"
 #include <math.h>
 #include <stdio.h>
 
@@ -58,6 +59,17 @@ struct AttnFwdParams {
   const int* doc_start;   // int32 [B, S], DOC kernels only: query s sees keys [doc_start[b, s], s]
 };
 
+// Dropout on the probabilities (DROP kernels only; DESIGN.md "Dropout"), a kernel parameter of its own so the parameter
+// blocks of the other instantiations stay as they are.  Local (b, h) is global batch b_off + rng[1] * b_micro + b and
+// global head h_off + h of H_glob; S_real is the unpadded sequence length.
+struct AttnDropParams {
+  unsigned long long seed;
+  const long long* rng;   // device [2]: optimizer step, pipeline micro-batch
+  long long b_off, b_micro;
+  int h_off, H_glob, S_real, site, thr;
+  float dscale;           // 256 / (256 - thr)
+};
+
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -65,10 +77,13 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 // DOC (document-masked causal attention): a query tile starts its KV loop at the tile holding the document start of its
 // first row (doc_start is non-decreasing along the sequence), and tiles below the document start of its last row get an
 // element mask.  A row can then see a fully masked tile, so the softmax subtracts 0 instead of a -inf running max.
-template <int HD, bool DOC>
+// DROP (dropout on P): the row max and sum (hence lse) come from the undropped P; the tile multiplied into V has the dropped
+// elements zeroed and O is scaled by 1 / keep probability at the end.  Mask call per (16-row block, 32-key block, row % 8,
+// (key % 8) / 2): the 16 elements (rows {g, g + 8} x 8 keys) a thread holds of that block.
+template <int HD, bool DOC, bool DROP>
 __global__ void __launch_bounds__(AttnCfg<HD>::THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                const __grid_constant__ CUtensorMap tmap_v, const AttnFwdParams p) {
+                const __grid_constant__ CUtensorMap tmap_v, const AttnFwdParams p, const AttnDropParams dr) {
   using L = FwdSmem<HD>;
   constexpr int KV_STAGES = AttnCfg<HD>::KV_STAGES;
   constexpr int NC = HD / 64;   // column chunks per row tile
@@ -141,6 +156,30 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     ds[1] = __ldg(dsb + row0 + 8);
     ds_last = __ldg(dsb + BQ - 1);
   }
+  // DROP: the step word, the counter row of this thread's row pair, and the other mask inputs
+  uint32_t drop_step = 0, drop_row = 0, drop_site = 0, drop_thr = 0;
+  unsigned long long drop_seed = 0;
+  if constexpr (DROP) {
+    drop_step = (uint32_t)dr.rng[0];
+    drop_site = (uint32_t)dr.site;
+    drop_thr = (uint32_t)dr.thr;
+    drop_seed = dr.seed;
+    const long long bg = dr.b_off + dr.rng[1] * dr.b_micro + b;
+    drop_row = (uint32_t)((bg * dr.H_glob + dr.h_off + h) * dr.S_real + qi * BQ + row0);
+  }
+  auto drop = [&](float (&s)[64], int j) {   // zero the dropped elements of P (fragment element 4 jj + 2 hr + e)
+#pragma unroll
+    for (int kb = 0; kb < 4; ++kb) {
+      const uint4 r = dropout::philox((uint32_t)(((j * 4 + kb) << 2) | q), drop_row, drop_step, drop_site, drop_seed);
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (dropout::byte_of(r, 8 * hr + 2 * u + e) < drop_thr) s[4 * (4 * kb + u) + 2 * hr + e] = 0.f;
+    }
+  };
   // online softmax of the score tile of KV tile j: s -> P (fp32), running max / sum updated, alpha = the factor O is rescaled by
   auto softmax = [&](float (&s)[64], int j, float (&alpha)[2]) {
     const bool diag = p.causal && j == qi;
@@ -186,6 +225,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       }
       l[hr] = l[hr] * alpha[hr] + sum;
     }
+    if constexpr (DROP) drop(s, j);
   };
   auto rescale_o = [&](const float (&alpha)[2]) {
 #pragma unroll
@@ -320,6 +360,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           o[4 * jj + 2 * hr + 1] *= alpha;
         }
       }
+      if constexpr (DROP) drop(s, j);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk) {
@@ -340,7 +381,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     float lsum = l[hr];
     lsum += __shfl_xor_sync(0xffffffffu, lsum, 1);
     lsum += __shfl_xor_sync(0xffffffffu, lsum, 2);
-    const float inv = 1.f / lsum;
+    const float inv = (DROP ? dr.dscale : 1.f) / lsum;
     const int row = qi * BQ + row0 + hr * 8;
     __nv_bfloat16* op = reinterpret_cast<__nv_bfloat16*>(p.O) + (((size_t)b * p.S + row) * p.H + h) * HD;
 #pragma unroll
@@ -402,11 +443,13 @@ struct AttnBwdParams {
 // key (binary search, doc_start is non-decreasing).  Inside the range P = 0 where key < doc_start[query]; since doc_start is
 // monotone, those queries are a suffix for each key row, so a thread keeps one bound per kv row instead of loading
 // doc_start per query column.
-template <int HD, bool DOC>
+// DROP: dV += (P Z)^T dO, dS = P (dP Z - delta).  The mask is regenerated from the forward's definition; a thread holds kv
+// rows {g, g + 8} (keys) x query columns, so it uses 4 bytes of each call: one call per (16-query block, query % 8 pair).
+template <int HD, bool DOC, bool DROP>
 __global__ void __launch_bounds__(AttnCfg<HD>::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
-                const AttnBwdParams p) {
+                const AttnBwdParams p, const AttnDropParams dr) {
   using L = BwdSmem<HD>;
   constexpr int Q_STAGES = AttnCfg<HD>::Q_STAGES;
   constexpr int NC = HD / 64;
@@ -507,11 +550,45 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
       qend[hr] = lo;
     }
   }
+  // Its inputs are recomputed per call from the thread / block indices and the parameter block, and the step / micro-batch
+  // words are loaded per call (volatile): the D = 128 loop has no registers to spare for copies kept across it.
+  auto keep_bits = [&](int i) {
+    uint32_t drop_step, micro;
+    asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(drop_step) : "l"(dr.rng));
+    asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(micro) : "l"(dr.rng + 1));
+    const uint32_t drop_c0 = (uint32_t)(((j * 4 + wg * 2 + ((warp >> 1) & 1)) << 2) | ((g >> 1) & 3));   // key column group
+    const uint32_t drop_row =   // counter row of query 0 of this (b, h)
+        (uint32_t)(((dr.b_off + (long long)micro * dr.b_micro + b) * dr.H_glob + dr.h_off + h) * dr.S_real);
+    uint32_t bits = 0;
+#pragma unroll
+    for (int jh = 0; jh < 4; ++jh)
+#pragma unroll
+      for (int e1 = 0; e1 < 2; ++e1) {
+        const uint4 r = dropout::philox(drop_c0, drop_row + i * BQB + 16 * jh + 2 * q + e1, drop_step, (uint32_t)dr.site, dr.seed);
+#pragma unroll
+        for (int jl = 0; jl < 2; ++jl) {
+          const uint32_t w = (warp & 1) ? (jl ? r.w : r.y) : (jl ? r.z : r.x);   // byte 8 jl + 4 (warp & 1) + 2 hr + (g & 1)
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr)
+            if (((w >> (8 * (2 * hr + (g & 1)))) & 0xffu) >= (uint32_t)dr.thr) bits |= 1u << (4 * (2 * jh + jl) + 2 * hr + e1);
+        }
+      }
+    return bits;
+  };
+  // x where element idx is kept, else 0 (bit operations only).  D = 64 applies the 1 / keep probability to dV once, when it
+  // is stored; D = 128 folds it into P Z.
+  auto keep = [](uint32_t bits, int idx, float x) { return __int_as_float(__float_as_int(x) & (0u - ((bits >> idx) & 1u))); };
   mbar_wait(kv_full, 0);
   for (int i = i0, it = 0; i < i_end; ++i, ++it) {
     const int st = it % Q_STAGES;
     mbar_wait(&q_full[st], (it / Q_STAGES) & 1);
     const uint32_t sq = smem_u32(smem + L::SB_Q + st * L::QB_BYTES), sdo = smem_u32(smem + L::SB_DO + st * L::QB_BYTES);
+    // at D = 128 the keep bits are formed before the S^T / dP^T accumulators are live (no registers for Philox beside them)
+    uint32_t kbits = 0;
+    if constexpr (DROP && HD == 128) {
+      kbits = keep_bits(i);
+      asm volatile("" : "+r"(kbits));   // pins the Philox work here, ahead of the MMAs below (ordered volatile asm)
+    }
     float s[32], dp[32];
     wgmma_fence();
 #pragma unroll
@@ -526,6 +603,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     wgmma_commit();
     const bool masked = p.causal && i * BQB < j * BKV + BKV;   // query block overlaps the kv block
     const bool dmask = DOC && i * BQB + BQB > min(qend[0], qend[1]);   // some query of the block is past a kv row's document
+    if constexpr (DROP && HD == 64) kbits = keep_bits(i);   // (while the MMAs run)
     if constexpr (HD == 64) {
       const float* stat = reinterpret_cast<const float*>(smem + L::SB_STAT + st * L::STAT_BYTES);
       wgmma_wait<1>();
@@ -551,7 +629,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {
         uint32_t a[4];
-        frag_a_from_acc(s, kk, a);
+        if constexpr (DROP) {
+#pragma unroll
+          for (int t = 0; t < 4; ++t)
+            a[t] = pack_bf16x2(keep(kbits, 8 * kk + 2 * t, s[8 * kk + 2 * t]), keep(kbits, 8 * kk + 2 * t + 1, s[8 * kk + 2 * t + 1]));
+        } else {
+          frag_a_from_acc(s, kk, a);
+        }
         wgmma_m64nXk16_bf16_rs<1>(dv, a, make_smem_desc_sw128(sdo + kk * 16 * 128, L::QB_CHUNK, 1024), 1u);
       }
       wgmma_commit();
@@ -565,7 +649,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
           for (int hr = 0; hr < 2; ++hr) {
             const int idx = 4 * jj + 2 * hr + e1;
-            dp[idx] = s[idx] * (dp[idx] - dl);
+            dp[idx] = s[idx] * ((DROP ? keep(kbits, idx, dp[idx]) * dr.dscale : dp[idx]) - dl);
           }
         }
       }
@@ -586,8 +670,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
           float pv = exp2f(s[idx] * p.scale_log2 - L2);
           if (masked && i * BQB + qt < j * BKV + wg * 64 + r0 + 8 * hr) pv = 0.f;
           if (dmask && i * BQB + qt >= qend[hr]) pv = 0.f;
-          s[idx] = pv;
-          dp[idx] = pv * (dp[idx] - dl);
+          if constexpr (DROP) {   // s = P Z (scaled here: dV needs no scaling at the end), dS = P Z dP - P delta
+            const float sz = keep(kbits, idx, pv) * dr.dscale;
+            dp[idx] = sz * dp[idx] - pv * dl;
+            s[idx] = sz;
+          } else {
+            s[idx] = pv;
+            dp[idx] = pv * (dp[idx] - dl);
+          }
         }
       }
     }
@@ -681,7 +771,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
 #pragma unroll
     for (int jj = 0; jj < HD / 8; ++jj) {
       *reinterpret_cast<uint32_t*>(dkp + 8 * jj + 2 * q) = pack_bf16x2(dk[4 * jj + 2 * hr] * p.scale, dk[4 * jj + 2 * hr + 1] * p.scale);
-      *reinterpret_cast<uint32_t*>(dvp + 8 * jj + 2 * q) = pack_bf16x2(dv[4 * jj + 2 * hr], dv[4 * jj + 2 * hr + 1]);
+      if constexpr (DROP && HD == 64)
+        *reinterpret_cast<uint32_t*>(dvp + 8 * jj + 2 * q) = pack_bf16x2(dv[4 * jj + 2 * hr] * dr.dscale, dv[4 * jj + 2 * hr + 1] * dr.dscale);
+      else
+        *reinterpret_cast<uint32_t*>(dvp + 8 * jj + 2 * q) = pack_bf16x2(dv[4 * jj + 2 * hr], dv[4 * jj + 2 * hr + 1]);
     }
   }
 }
@@ -782,9 +875,29 @@ cudaError_t set_smem(int bytes) {   // once per kernel instantiation
   return cudaSuccess;
 }
 
+
+template <int HD, bool DOC, bool DROP>
+int launch_fwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnFwdParams& p, const AttnDropParams& dr,
+               cudaStream_t stream) {
+  cudaError_t e = set_smem<attn_fwd_kernel<HD, DOC, DROP>>(FwdSmem<HD>::BYTES);
+  if (e != cudaSuccess) return (int)e;
+  return (int)tepd::launch(attn_fwd_kernel<HD, DOC, DROP>, dim3((p.S / BQ) * p.B * p.H), dim3(AttnCfg<HD>::THREADS), FwdSmem<HD>::BYTES,
+                           stream, tq, tk, tv, p, dr);
+}
+
+template <int HD, bool DOC, bool DROP>
+cudaError_t launch_bwd(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo, const AttnBwdParams& p,
+                       const AttnDropParams& dr, cudaStream_t st) {
+  cudaError_t e = set_smem<attn_bwd_kernel<HD, DOC, DROP>>(BwdSmem<HD>::BYTES);
+  if (e != cudaSuccess) return e;
+  return tepd::launch(attn_bwd_kernel<HD, DOC, DROP>, dim3((p.S / BKV) * p.B * p.H), dim3(AttnCfg<HD>::THREADS), BwdSmem<HD>::BYTES, st,
+                      tq, tk, tv, tdo, p, dr);
+}
+
 template <int HD>
 int attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, int B, int H, int S, float scale, int causal,
-             long long stride_b, long long stride_s, long long stride_h, const int* doc_start, cudaStream_t stream) {
+             long long stride_b, long long stride_s, long long stride_h, const int* doc_start, const AttnDropParams& drop,
+             cudaStream_t stream) {
   CUtensorMap tq, tk, tv;
   int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, HD, stride_b, stride_s, stride_h, BQ);
   if (rc) return 100 + rc;
@@ -792,23 +905,20 @@ int attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, in
   if (rc) return 200 + rc;
   rc = tepd_make_tmap_bshd(&tv, v, B, S, H, HD, stride_b, stride_s, stride_h, BKV);
   if (rc) return 300 + rc;
-  auto kern = doc_start ? attn_fwd_kernel<HD, true> : attn_fwd_kernel<HD, false>;
-  cudaError_t e = doc_start ? set_smem<attn_fwd_kernel<HD, true>>(FwdSmem<HD>::BYTES)
-                            : set_smem<attn_fwd_kernel<HD, false>>(FwdSmem<HD>::BYTES);
-  if (e != cudaSuccess) return (int)e;
   AttnFwdParams p;
   p.O = o; p.lse = (float*)lse; p.B = B; p.H = H; p.S = S; p.causal = causal;
   p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   p.doc_start = doc_start;
-  return (int)tepd::launch(kern, dim3((S / BQ) * B * H), dim3(AttnCfg<HD>::THREADS), FwdSmem<HD>::BYTES, stream,
-                           tq, tk, tv, p);
+  if (!drop.rng)
+    return doc_start ? launch_fwd<HD, true, false>(tq, tk, tv, p, drop, stream) : launch_fwd<HD, false, false>(tq, tk, tv, p, drop, stream);
+  return doc_start ? launch_fwd<HD, true, true>(tq, tk, tv, p, drop, stream) : launch_fwd<HD, false, true>(tq, tk, tv, p, drop, stream);
 }
 
 template <int HD>
 int attn_bwd(const void* dO, const void* q, const void* k, const void* v, const void* o, const void* lse, float* delta,
              float* dq_acc, void* dq, void* dk, void* dv, int B, int H, int S, float scale, int causal, long long stride_b,
              long long stride_s, long long stride_h, long long dstride_b, long long dstride_s, long long dstride_h,
-             const int* doc_start, cudaStream_t st) {
+             const int* doc_start, const AttnDropParams& drop, const int* zero_docs, cudaStream_t st) {
   CUtensorMap tq, tk, tv, tdo;
   int rc = tepd_make_tmap_bshd(&tq, q, B, S, H, HD, stride_b, stride_s, stride_h, BQB);
   if (rc) return 100 + rc;
@@ -824,17 +934,27 @@ int attn_bwd(const void* dO, const void* q, const void* k, const void* v, const 
                                   (const __nv_bfloat16*)dO, (const __nv_bfloat16*)o, delta, B, S, H);
     if (le != cudaSuccess) return (int)le;
   }
-  auto kern = doc_start ? attn_bwd_kernel<HD, true> : attn_bwd_kernel<HD, false>;
-  cudaError_t e = doc_start ? set_smem<attn_bwd_kernel<HD, true>>(BwdSmem<HD>::BYTES)
-                            : set_smem<attn_bwd_kernel<HD, false>>(BwdSmem<HD>::BYTES);
-  if (e != cudaSuccess) return (int)e;
   AttnBwdParams p;
   p.lse = (const float*)lse; p.delta = delta; p.dq_acc = dq_acc; p.dk = dk; p.dv = dv;
   p.dstride_b = dstride_b; p.dstride_s = dstride_s; p.dstride_h = dstride_h;
   p.B = B; p.H = H; p.S = S; p.causal = causal; p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   p.doc_start = doc_start;
-  cudaError_t le = tepd::launch(kern, dim3((S / BKV) * B * H), dim3(AttnCfg<HD>::THREADS), BwdSmem<HD>::BYTES, st,
-                                tq, tk, tv, tdo, p);
+  cudaError_t le;
+  if (!drop.rng) {
+    le = doc_start ? launch_bwd<HD, true, false>(tq, tk, tv, tdo, p, drop, st) : launch_bwd<HD, false, false>(tq, tk, tv, tdo, p, drop, st);
+  } else if constexpr (HD == 128) {
+    // D = 128 with dropout always runs the DOC instantiation: the other one does not fit the 240-register budget of its
+    // consumers.  Without document masks every "document" starts at 0 (a zeroed int32 [B, S]), which masks nothing -- for
+    // non-causal attention too: the query-block range and the per-row bounds the DOC kernel derives from it are then the
+    // whole sequence.  The caller owns that buffer (`zero_docs`), so a captured graph never outlives it.
+    if (!doc_start) {
+      if (!zero_docs) return -2;
+      p.doc_start = zero_docs;
+    }
+    le = launch_bwd<HD, true, true>(tq, tk, tv, tdo, p, drop, st);
+  } else {
+    le = doc_start ? launch_bwd<HD, true, true>(tq, tk, tv, tdo, p, drop, st) : launch_bwd<HD, false, true>(tq, tk, tv, tdo, p, drop, st);
+  }
   if (le != cudaSuccess) return (int)le;
   return (int)tepd::launch(attn_dq_cast_kernel<HD>, dim3(tepd::num_sms() * 4), dim3(256), 0, st, dq_acc, (__nv_bfloat16*)dq, B, S,
                            H, dstride_b, dstride_s, dstride_h);
@@ -844,24 +964,35 @@ int attn_bwd(const void* dO, const void* q, const void* k, const void* v, const 
 
 // q, k, v: bf16 pointers addressed as [B, S, H, D] with the given element strides (shared by q/k/v).  D = 64 or 128.
 // doc_start: nullptr, or int32 [B, S] non-decreasing document starts (causal only): query s sees keys [doc_start[b, s], s].
+// rng: nullptr (no dropout), or the device int64 [2] (optimizer step, pipeline micro-batch) of dropout on the probabilities
+// with threshold byte thr (p = thr / 256), Philox key seed and site id; this call's (b, h) are global batch
+// b_off + rng[1] * b_micro + b and global head h_off + h of H_glob, and S_real <= S is the unpadded sequence length.
 extern "C" int tepd_attn_fwd(const void* q, const void* k, const void* v, void* o, void* lse, int B, int H, int S, int D,
                              float scale, int causal, long long stride_b, long long stride_s, long long stride_h,
-                             void* stream, const int* doc_start) {
+                             void* stream, const int* doc_start, unsigned long long seed, const void* rng, long long b_off,
+                             long long b_micro, int h_off, int H_glob, int S_real, int site, int thr) {
   if (S % 128 != 0 || (doc_start && !causal)) return -2;
+  if (rng && (thr < 0 || thr > 255 || S_real > S || H_glob < H)) return -2;
+  const AttnDropParams drop = {seed, (const long long*)rng, b_off, b_micro, h_off, H_glob, S_real, site, thr, 256.f / (float)(256 - thr)};
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (D == 64) return attn_fwd<64>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, doc_start, st);
-  if (D == 128) return attn_fwd<128>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, doc_start, st);
+  if (D == 64) return attn_fwd<64>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, doc_start, drop, st);
+  if (D == 128) return attn_fwd<128>(q, k, v, o, lse, B, H, S, scale, causal, stride_b, stride_s, stride_h, doc_start, drop, st);
   return -2;
 }
 
 // do, o: contiguous [B,S,H,D]; q/k/v strided views; dq/dk/dv strided views (shared strides).  D = 64 or 128.
 // lse: contiguous fp32 [B, H, S] (16-byte aligned at D = 64).  dq_acc: nullptr (a persistent, self-clearing workspace of the
 // library's) or a zeroed fp32 buffer of B * S * H * D elements in the layout attn_dq_cast_kernel reads; left zeroed.
+// zero_docs: with dropout (rng) at D = 128 and no doc_start, a caller-owned int32 [B, S] of zeros (see attn_bwd); else unused.
 extern "C" int tepd_attn_bwd(const void* dO, const void* q, const void* k, const void* v, const void* o, const void* lse,
                              void* dq_acc, void* dq, void* dk, void* dv, int B, int H, int S, int D, float scale,
                              int causal, long long stride_b, long long stride_s, long long stride_h, long long dstride_b,
-                             long long dstride_s, long long dstride_h, void* stream, const int* doc_start) {
+                             long long dstride_s, long long dstride_h, void* stream, const int* doc_start,
+                             unsigned long long seed, const void* rng, long long b_off, long long b_micro, int h_off, int H_glob,
+                             int S_real, int site, int thr, const int* zero_docs) {
   if ((D != 64 && D != 128) || S % 128 != 0 || (doc_start && !causal)) return -2;
+  if (rng && (thr < 0 || thr > 255 || S_real > S || H_glob < H)) return -2;
+  const AttnDropParams drop = {seed, (const long long*)rng, b_off, b_micro, h_off, H_glob, S_real, site, thr, 256.f / (float)(256 - thr)};
   if (D == 64 && (reinterpret_cast<uintptr_t>(lse) & 15)) return -2;   // lse rows are bulk-copied (16-byte alignment)
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   static float* delta_buf = nullptr;
@@ -887,7 +1018,7 @@ extern "C" int tepd_attn_bwd(const void* dO, const void* q, const void* k, const
   }
   if (D == 64)
     return attn_bwd<64>(dO, q, k, v, o, lse, delta_buf, (float*)dq_acc, dq, dk, dv, B, H, S, scale, causal, stride_b, stride_s,
-                        stride_h, dstride_b, dstride_s, dstride_h, doc_start, st);
+                        stride_h, dstride_b, dstride_s, dstride_h, doc_start, drop, zero_docs, st);
   return attn_bwd<128>(dO, q, k, v, o, lse, delta_buf, (float*)dq_acc, dq, dk, dv, B, H, S, scale, causal, stride_b, stride_s,
-                       stride_h, dstride_b, dstride_s, dstride_h, doc_start, st);
+                       stride_h, dstride_b, dstride_s, dstride_h, doc_start, drop, zero_docs, st);
 }

@@ -5,6 +5,7 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 #include "launch.cuh"
+#include "dropout_philox.cuh"
 
 namespace {
 
@@ -608,6 +609,39 @@ __global__ void __launch_bounds__(256) ew_bf16_kernel(const uint4* __restrict__ 
     out[i] = pack8(o);
   }
 }
+// ---- dropout (DESIGN.md "Dropout"): y = x * Z (forward, and the backward of any dropout: it applies the same mask) or, ADD,
+// y = res + x * Z.  x / res / y are this shard's contiguous [A, R, C] view of a tensor whose global row of (a, r) is
+// (a_off + rng[1] * a_micro + a) * Rg + r_off + r and whose global column of c is c_off + c.  rng[0] is the optimizer step and
+// rng[1] the pipeline micro-batch: both are read from device memory, so a captured CUDA graph sees the current values.
+// One Philox call per 16 columns (a thread's two 16-byte vectors).
+template <bool ADD>
+__global__ void __launch_bounds__(256) dropout_kernel(const uint4* __restrict__ x, const uint4* __restrict__ res, uint4* __restrict__ y,
+                                                      long long units, int R, int C16, long long a_off, long long a_micro,
+                                                      long long r_off, long long Rg, long long c16_off, unsigned long long seed,
+                                                      const long long* __restrict__ rng, int site, int thr, float scale) {
+  pdl_wait();
+  const uint32_t step = (uint32_t)rng[0];
+  const long long a_base = a_off + rng[1] * a_micro;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < units; i += (long long)gridDim.x * blockDim.x) {
+    const long long row = i / C16;
+    const int cg = (int)(i - row * C16);
+    const long long a = row / R;
+    const long long grow = (a_base + a) * Rg + r_off + (row - a * R);
+    const uint4 bits = dropout::philox((uint32_t)(c16_off + cg), (uint32_t)grow, step, (uint32_t)site, seed);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float v[8], rv[8];
+      unpack8(__ldg(x + 2 * i + h), v);
+      if (ADD) unpack8(__ldg(res + 2 * i + h), rv);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        v[e] = dropout::byte_of(bits, 8 * h + e) >= (uint32_t)thr ? v[e] * scale : 0.f;
+        if (ADD) v[e] += rv[e];
+      }
+      y[2 * i + h] = pack8(v);
+    }
+  }
+}
 // 8 elements per thread: two 16-byte loads, one 16-byte store (pointers 32 / 16-byte aligned, n % 8 == 0)
 __global__ void __launch_bounds__(256) cast_f32_bf16_vec_kernel(const float4* __restrict__ in, uint4* __restrict__ out, size_t nvec) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < nvec; i += (size_t)gridDim.x * blockDim.x) {
@@ -792,6 +826,22 @@ extern "C" int tepd_ew_bf16(const void* a, const void* b, void* out, long long n
   if (mode == 0) return (int)tepd::launch(ew_bf16_kernel<0>, grid, dim3(256), 0, CS(stream), (const uint4*)a, (const uint4*)b, (uint4*)out, nvec);
   if (mode == 1) return (int)tepd::launch(ew_bf16_kernel<1>, grid, dim3(256), 0, CS(stream), (const uint4*)a, (const uint4*)b, (uint4*)out, nvec);
   return (int)tepd::launch(ew_bf16_kernel<2>, grid, dim3(256), 0, CS(stream), (const uint4*)a, (const uint4*)b, (uint4*)out, nvec);
+}
+// Dropout of a contiguous bf16 [A, R, C] shard (see dropout_kernel): res == nullptr -> y = x * Z, else y = res + x * Z.
+// C % 16 == 0, c_off % 16 == 0, pointers 16-byte aligned.
+extern "C" int tepd_dropout(const void* x, const void* res, void* y, long long A, int R, int C, long long a_off, long long a_micro,
+                            long long r_off, long long Rg, long long c_off, unsigned long long seed, const void* rng, int site,
+                            int thr, float scale, void* stream) {
+  if (C % 16 || c_off % 16 || A <= 0 || R <= 0 || thr < 0 || thr > 255 || !rng ||
+      ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(res)) & 15))
+    return -2;
+  const long long units = A * R * (C / 16);
+  dim3 grid(grid_for((size_t)units, 256));
+  if (res)
+    return (int)tepd::launch(dropout_kernel<true>, grid, dim3(256), 0, CS(stream), (const uint4*)x, (const uint4*)res, (uint4*)y, units,
+                             R, C / 16, a_off, a_micro, r_off, Rg, c_off / 16, seed, (const long long*)rng, site, thr, scale);
+  return (int)tepd::launch(dropout_kernel<false>, grid, dim3(256), 0, CS(stream), (const uint4*)x, (const uint4*)x, (uint4*)y, units,
+                           R, C / 16, a_off, a_micro, r_off, Rg, c_off / 16, seed, (const long long*)rng, site, thr, scale);
 }
 extern "C" int tepd_attn_merge(void* o_acc, const void* lse_in, void* lse_out, const void* o_j, const void* lse_j, int B, int L, int H,
                                int D, int first, void* stream) {

@@ -289,6 +289,9 @@ def check_context_parallel(graph: Graph, strategy: str) -> None:
     if wants_cp and any(n.op == "attention" and len(n.inputs) > 1 for n in graph.nodes):
         raise ValueError(f"strategy {strategy!r}: context parallelism does not support document-masked attention "
                          "(eot_token / doc_starts); use dp, tp, pp or auto")
+    if wants_cp and any(n.op == "attention" and float(n.attrs.get("pdrop", 0.0)) > 0 for n in graph.nodes):
+        raise ValueError(f"strategy {strategy!r}: context parallelism does not support attention dropout (attn_pdrop > 0: the "
+                         "ring's block kernels have no global query / key offsets); use dp, tp, pp or auto")
 
 
 def plan_and_build(graph: Graph, trainer, strategy: str, comm_mode: str, use_cuda_graph: bool, seed: int):

@@ -40,6 +40,7 @@ _TORCH_DTYPE = {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float
                 "i64": torch.int64, "bool": torch.bool}
 _ALIGN = 128  # elements; keeps every variable slice 16-B aligned in every dtype
 FLAT_APPLY = ("apply_adamw", "apply_sgd")   # elementwise updates: may run over the flat buffers / fused sharded-optimizer kernels
+DROPOUT_OPS = ("dropout", "dropout_bwd", "dropout_add")
 
 
 def torch_dtype(name: str, device: torch.device) -> torch.dtype:
@@ -242,6 +243,19 @@ class Executor:
             collective.dry = True
         self.step_count = 0
         self._tag = 0   # micro-batch tag for per-micro-batch side tables (pipeline interleaves micro-batches)
+        # dropout (DESIGN.md "Dropout"): the masks are keyed by the seed and read (step, micro-batch) from this device tensor,
+        # written per step by _set_hyper (and per micro-batch by a pipeline stage), so captured CUDA graphs stay correct
+        self.has_dropout = any(n.op in DROPOUT_OPS or float(n.attrs.get("pdrop", 0.0)) > 0 for n in graph.nodes)
+        self.drop_seed = int(seed)
+        self.rng_state = torch.zeros(2, dtype=torch.int64, device=self.device)
+        self.drop_state = self.rng_state      # what the dropout kernels read (a pipeline stage points it at a slot's copy)
+        self.micro_level: Optional[int] = None   # pipeline micro-batch level: its cuts move the offsets by rng_state[1]
+        if self.device.type == "cuda":
+            for n in graph.nodes:    # what dropout_kernel takes: refused here rather than at the first step
+                t = n.outputs[0] if n.op in DROPOUT_OPS else None
+                if t is not None and (t.dtype != "bf16" or not t.shape or t.shape[-1] % 16):
+                    raise ValueError(f"{n.op} '{n.name}': the GPU dropout kernel takes bf16 tensors whose last dim (per shard) is a "
+                                     f"multiple of 16; got {t.dtype} {tuple(t.shape)}")
         self.use_cuda_graph = use_cuda_graph and self.device.type == "cuda"
         if self.use_cuda_graph and any(n.attrs.get("cp_levels") for n in graph.nodes) and os.environ.get("TEPDIST_CP_GRAPH") != "1":
             self.use_cuda_graph = False    # ring attention posts point-to-point batches per block: run the step eagerly
@@ -708,6 +722,8 @@ class Executor:
         return self._static_out
 
     def _set_hyper(self) -> None:
+        if self.has_dropout:
+            self.rng_state[0].fill_(self.step_count)
         kind = self.opt.get("kind")
         lr = self.lr_fn(self.step_count) if self.lr_fn else self.opt.get("lr", 1e-3)
         lr = 0.0 if lr is None else float(lr)      # (lr=None: Adafactor's relative step size, hyper[H_AF_REL_LR])
@@ -1000,6 +1016,24 @@ class Executor:
         elif pc is None and comp.data_ptr() != master.data_ptr():
             comp.copy_(master.to(comp.dtype))
         env[(n.id, 0)] = comp if comp.is_contiguous() else comp.contiguous()
+
+    def _drop_rng(self, n: Node) -> "ops.DropoutRng":
+        """Mask source of dropout-bearing node `n`: its site, and where this rank's output shard sits in the global tensor,
+        from the cuts the transform recorded (drop_dims / drop_nums / drop_levels of the unsharded drop_full) and this rank's
+        mesh coordinates.  The pipeline's micro-batch level contributes through rng_state[1] instead of a coordinate."""
+        a = n.attrs
+        full = [int(d) for d in a.get("drop_full", n.outputs[0].shape)]
+        size, off, mic = list(full), [0] * len(full), [0] * len(full)
+        for d, k, lvl in zip(a.get("drop_dims", []), a.get("drop_nums", []), a.get("drop_levels", [])):
+            d, k, lvl = int(d), int(k), int(lvl)
+            size[d] //= k
+            if self.micro_level is not None and lvl == self.micro_level:
+                mic[d] += size[d]
+            else:
+                off[d] += self.coords.get(lvl, 0) * size[d]
+        if n.op == "attention_bwd":     # dqkv [B, S, 3C]: dim 2 in units of the forward's [B, S, C] output
+            full[2], off[2], mic[2] = full[2] // 3, off[2] // 3, mic[2] // 3
+        return ops.DropoutRng(self.drop_seed, self.drop_state, int(a["site"]), tuple(off), tuple(mic), tuple(full))
 
     def _ring(self, n: Node):
         """The K / V ring of a context-parallel attention node (transform.cc stamps `cp_levels` on "seq" candidates), or None."""
@@ -1392,6 +1426,8 @@ class Executor:
             out = self._grad_out(n, 0, n.outputs[0].shape)
             ops.colsum_acc(ins[0], out)
             return [out]
+        if op in DROPOUT_OPS:
+            return [ops.dropout(ins[0], a["p"], self._drop_rng(n), ins[1] if op == "dropout_add" else None)]
         if op == "gelu":
             return [ops.gelu_fwd(ins[0].contiguous())]
         if op == "gelu_bwd":
@@ -1403,18 +1439,22 @@ class Executor:
             D = C3 // 3 // H
             q5 = qkv.view(B, S, H, 3, D)  # heads-major: a last-dim split is a split over heads
             ds = ins[1] if len(ins) > 1 else None
+            pdrop = float(a.get("pdrop", 0.0))
             ring = self._ring(n)
             if ring is not None:    # context parallel: S is this rank's block of the sequence, K / V blocks ride the ring
                 if ds is not None:
                     raise NotImplementedError("context parallelism (K / V ring) with document-masked attention")
+                if pdrop:
+                    raise NotImplementedError("context parallelism (K / V ring) with attention dropout")
                 o, lse = ring.forward(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], causal=a.get("causal", True))
                 return [o.reshape(B, S, H * D), lse]
             o, lse = ops.attention_fwd(q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], causal=a.get("causal", True),
-                                       doc_start=ds)
+                                       doc_start=ds, pdrop=pdrop, rng=self._drop_rng(n) if pdrop else None)
             return [o.view(B, S, H * D), lse]
         if op == "attention_bwd":
             do, qkv, o, lse = ins[:4]
             ds = ins[4] if len(ins) > 4 else None
+            pdrop = float(a.get("pdrop", 0.0))
             B, S, C3 = qkv.shape
             H = a["heads"]
             D = C3 // 3 // H
@@ -1424,11 +1464,14 @@ class Executor:
             if ring is not None:
                 if ds is not None:
                     raise NotImplementedError("context parallelism (K / V ring) with document-masked attention")
+                if pdrop:
+                    raise NotImplementedError("context parallelism (K / V ring) with attention dropout")
                 ring.backward(do.reshape(B, S, H, D), q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], o.reshape(B, S, H, D), lse,
                               causal=a.get("causal", True), dqkv_out=dqkv)
                 return [dqkv.view(B, S, C3)]
             ops.attention_bwd(do.reshape(B, S, H, D), q5[:, :, :, 0], q5[:, :, :, 1], q5[:, :, :, 2], o.reshape(B, S, H, D),
-                              lse, causal=a.get("causal", True), dqkv_out=dqkv, doc_start=ds)
+                              lse, causal=a.get("causal", True), dqkv_out=dqkv, doc_start=ds, pdrop=pdrop,
+                              rng=self._drop_rng(n) if pdrop else None)
             return [dqkv.view(B, S, C3)]
         if op == "softmax_xent":
             logits, labels = ins

@@ -98,6 +98,8 @@ class StageWorker:
         self.sub, self.idmap = self._extract(g, mine)
         self.exec = Executor(self.sub, device, seed=seed, collective=collective, coords=dict(coords or {}), comm_mode=comm_mode)
         self.exec.grad_accumulate = True    # gradients accumulate over micro-batches: atomically-added, zero-filled slots
+        self.exec.micro_level = micro_level if num_micro > 1 else None
+        self._slot_rng: Dict[int, torch.Tensor] = {}   # dropout (step, micro-batch) words read by slot k's captured bodies
         spmd = 1
         if collective is not None:
             spmd = max(1, collective.mesh.world // max(1, num_stages))
@@ -247,11 +249,29 @@ class StageWorker:
                     free.append(slot_of[dead])
         self.slot_of, self.num_slots = slot_of, n
 
+    def _drop_state(self, slot: Optional[int], m: int) -> None:
+        """Point the dropout kernels at the (step, micro-batch) words for micro-batch m: the executor's own for an eager body,
+        slot k's fixed-address copy for a captured one (a replay for another micro-batch then reads that micro-batch's index,
+        staged here like the inputs, not the one frozen at capture)."""
+        ex = self.exec
+        if not ex.has_dropout:
+            return
+        if slot is None:
+            st = ex.rng_state
+        else:
+            st = self._slot_rng.get(slot)
+            if st is None:
+                st = self._slot_rng[slot] = torch.zeros(2, dtype=torch.int64, device=ex.device)
+            st[0].fill_(ex.step_count)
+        st[1].fill_(m)
+        ex.drop_state = st
+
     def _stage_feeds(self, slot: int, m: int, feeds: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
         """Per-slot staging of the fed inputs this stage consumes: micro-batch m's shard is copied into a fixed buffer (the
         captured body reads that address)."""
         ex = self.exec
         ex.coords[self.micro_level] = m
+        self._drop_state(slot, m)
         out = self._static_feeds.setdefault(slot, {})
         dev = ex.device
         for n in self.sub.nodes:
@@ -275,6 +295,7 @@ class StageWorker:
     def _run_phase(self, bwd: bool, m: int, feeds: Dict[str, torch.Tensor]) -> None:
         nodes = self.bwd_nodes if bwd else self.fwd_nodes
         if not self.use_graph or self.steps_run < 1 or m not in self.slot_of:
+            self._drop_state(None, m)
             self._run_nodes(nodes, m, feeds)          # eager (first step = warm-up: lazy allocations, kernel attributes)
             return
         slot = self.slot_of[m]
