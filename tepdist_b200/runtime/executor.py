@@ -62,7 +62,7 @@ class VariableStore:
     """Flat device-resident storage for all variables of a graph (+ grads and optimizer slots)."""
 
     def __init__(self, graph: Graph, device: torch.device, seed: int = 0, coords: Optional[Dict[int, int]] = None,
-                 tail: Optional[set] = None):
+                 tail: Optional[set] = None, tail_align: int = _ALIGN):
         self.device = device
         self.coords = coords or {}
         tail = tail or set()
@@ -78,6 +78,10 @@ class VariableStore:
         off = 0
         self.n_decay = 0
         for n in params:
+            if n.id in tail and off == self.regular_end:
+                # the tail starts on a multiple of `tail_align` (the executor passes data-parallel degree x _ALIGN), so
+                # the flat sharded optimizer can split the whole regular range into equal per-rank chunks
+                off = self.regular_end = (off + tail_align - 1) // tail_align * tail_align
             self.offset[n.id] = off
             self.shape[n.id] = tuple(n.outputs[0].shape)
             self.cdtype[n.id] = n.outputs[0].dtype
@@ -219,6 +223,94 @@ class VariableStore:
         self.sync_compute()
 
 
+class FlatZeroLayout:
+    """Where the flat sharded optimizer (data-parallel ZeRO-1 over the flat buffers) updates, over `num` ranks.
+
+    `ranges` lists every sharded flat range as (start, end, n_decay, local_grad): first the gradient buckets in buffer order
+    (bucket i is ranges[i]), then one range per replicated-gradient variable.  Rank r owns the r-th of `num` equal chunks of
+    each range.  `n_decay` is a GLOBAL flat prefix length: element e decays iff e < n_decay.  For the buckets it is the
+    store's decayed prefix (VariableStore puts decayed variables first); for a replicated variable at [off, off + numel) it is
+    off + numel when the variable decays and off when it does not.  `local_grad`: the gradient of the range is complete on
+    every rank (computed redundantly), so the update reads the local gradient instead of summing the peers'."""
+
+    def __init__(self, num: int, total: int, ranges: List[Tuple[int, int, int, bool]], n_buckets: int,
+                 ready_at: Dict[int, List[int]], replicated: Dict[int, Tuple[int, int, int, bool]]):
+        self.num = num
+        self.total = total                # length the flat buffers need (the regular range padded to whole chunks)
+        self.ranges = ranges
+        self.n_buckets = n_buckets
+        self.ready_at = ready_at          # gradient producer node (-1: none) -> buckets complete once it has run
+        self.replicated = replicated      # apply node -> (variable, offset, numel, decay), in the order of ranges[n_buckets:]
+
+    @property
+    def buckets(self) -> List[Tuple[int, int]]:
+        return [(s0, e0) for s0, e0, _, _ in self.ranges[:self.n_buckets]]
+
+    def call(self, i: int, r: int) -> Tuple[int, int, int, bool]:
+        """(begin, end, n_decay, local_grad) of rank r's update of ranges[i]."""
+        s0, e0, nd, local = self.ranges[i]
+        chunk = (e0 - s0) // self.num
+        return s0 + r * chunk, s0 + (r + 1) * chunk, nd, local
+
+    def order(self) -> List[int]:
+        """Indices into `ranges` in the order a rank issues their updates: the buckets as backward completes them, then the
+        replicated variables (whose gradients are the last thing backward produces)."""
+        return [bi for k in sorted(self.ready_at) for bi in self.ready_at[k]] + list(range(self.n_buckets, len(self.ranges)))
+
+    def calls(self, r: int) -> List[Tuple[int, int, int, bool]]:
+        return [self.call(i, r) for i in self.order()]
+
+    @staticmethod
+    def local_decay(begin: int, end: int, n_decay: int) -> int:
+        """The decayed prefix length of the slice [begin, end), for ops.adamw_step on that slice."""
+        return min(max(n_decay - begin, 0), end - begin)
+
+
+def flat_zero_layout(store: VariableStore, fz: Dict[str, Any], num: int, opt: Dict[str, Any]) -> Optional[FlatZeroLayout]:
+    """The flat sharded-optimizer layout of `store` under the static analysis `fz` (Executor._analyze_flat_zero), or None
+    when the regular variables cannot all be covered by whole per-rank chunks (those plans keep the general per-tensor path).
+    Pure: reads the store's offsets and changes nothing; the caller grows the buffers to `total`."""
+    st = store
+    gran = num * _ALIGN
+    total = st.total
+    end = (st.regular_end + gran - 1) // gran * gran
+    if end > st.regular_end:
+        if st.regular_end != st.total:   # irregular tail present: the range cannot be padded in the middle of the buffers
+            end = st.regular_end // gran * gran
+        else:
+            total = end
+    numel = {p: int(torch.Size(st.shape[p]).numel()) for p in st.order}
+    offs = sorted((st.offset[p], p) for p in st.order if p not in fz["irregular_params"])
+    # a variable can only be covered whole: one that reaches past `end` (after it, or straddling it) sends every
+    # variable to the general path
+    if not offs or any(o + numel[p] > end for o, p in offs):
+        return None
+    # graded bucket sizes: the variables at the front of the flat buffer belong to the first layers, whose gradients
+    # are produced LAST by the backward pass -- whatever is still in flight when backward ends is exposed, so the
+    # buckets that become ready last are small (4M elements, doubling up to bucket_elems)
+    bucket_elems = int(opt.get("bucket_elems", 48 * 1024 * 1024))
+    first = int(opt.get("first_bucket_elems", os.environ.get("TEPDIST_FIRST_BUCKET", 4 * 1024 * 1024)))
+    from .. import _C
+    # (the bucket policy lives in the C++ core next to the gradient-collective combiner: csrc/transform.cc PlanFlatBuckets)
+    bounds = list(_C.plan_flat_buckets([int(off) for off, _ in offs], int(end), int(gran), int(first), int(bucket_elems)))
+    ranges = [(bounds[i], bounds[i + 1], st.n_decay, False) for i in range(len(bounds) - 1)]
+    prod_of_param = {pid: key[0] for key, pid in fz["binding"].items()}
+    ready_at: Dict[int, List[int]] = {}
+    for bi, (s0, e0, _, _) in enumerate(ranges):
+        last = max((prod_of_param[p] for off, p in offs if s0 <= off < e0 and p in prod_of_param), default=-1)
+        ready_at.setdefault(last, []).append(bi)
+    # replicated-gradient variables: the update is still sharded when every rank's chunk is a whole number of float4s
+    rep: Dict[int, Tuple[int, int, int, bool]] = {}
+    if opt.get("kind") == "adamw":
+        for aid, (pid, _gkey, decay) in fz.get("replicated", {}).items():
+            off, n_el = st.offset[pid], numel[pid]
+            if n_el % (4 * num) == 0 and off % 4 == 0:
+                rep[aid] = (pid, off, n_el, decay)
+    n_buckets = len(ranges)
+    ranges += [(off, off + n_el, off + n_el if decay else off, True) for (_, off, n_el, decay) in rep.values()]
+    return FlatZeroLayout(num, total, ranges, n_buckets, ready_at, rep)
+
+
 class Executor:
     """Interprets a Graph on one device.  `grad_sync(flat_grad)` (optional) is called once between the
     backward and the optimizer nodes — the data-parallel hook (see parallel/dp.py)."""
@@ -233,7 +325,8 @@ class Executor:
         self.comm_mode = comm_mode
         self._fz_static = self._analyze_flat_zero(graph) if collective is not None else None
         tail = self._fz_static["irregular_params"] if self._fz_static else set()
-        self.store = store or VariableStore(graph, self.device, seed, self.coords, tail=tail)
+        tail_align = self._fz_static["num"] * _ALIGN if self._fz_static else _ALIGN
+        self.store = store or VariableStore(graph, self.device, seed, self.coords, tail=tail, tail_align=tail_align)
         self.grad_sync = grad_sync
         self.collective = collective
         # timing-only mode (bench.py's exposed-communication measurement): every collective is replaced by a local
@@ -432,7 +525,7 @@ class Executor:
         binding: Dict[Tuple[int, int], int] = {}
         regular_apply: set = set()
         irregular_params: set = set()
-        replicated: Dict[int, Tuple[int, Tuple[int, int]]] = {}   # apply node -> (param, gradient value)
+        replicated: Dict[int, Tuple[int, Tuple[int, int], bool]] = {}   # AdamW apply node -> (param, gradient value, decay)
         level = num = None
         for a in apply_nodes:
             nd = g.nodes[a.inputs[0].node]
@@ -460,9 +553,9 @@ class Executor:
                     irregular_params.add(root)
                     # whole variable, whole slots, gradient computed redundantly on every rank (no collective in front of
                     # the apply): the update can still be sharded -- owner updates its chunk and stores it to every peer
-                    if (nd.op == "parameter" and c.op not in COLLECTIVE_OPS and "shard_dims" not in nd.attrs
+                    if (a.op == "apply_adamw" and nd.op == "parameter" and c.op not in COLLECTIVE_OPS and "shard_dims" not in nd.attrs
                             and all(g.nodes[v.node].op == "state" for v in a.inputs[2:])):
-                        replicated[a.id] = (root, a.inputs[1].key())
+                        replicated[a.id] = (root, a.inputs[1].key(), bool(a.attrs.get("decay", True)))
                 continue
             binding[c.inputs[0].key()] = pid
             regular_apply.add(a.id)
@@ -492,69 +585,27 @@ class Executor:
         fz = self._fz_static
         if fz is None:
             return
-        g, st = self.g, self.store
+        st = self.store
         if self.opt.get("kind") == "adamw":
             st.ensure_slots(flat_moments=True)      # the chunked update addresses m / v by flat offset
         num = fz["num"]
-        bucket_elems = int(self.opt.get("bucket_elems", 48 * 1024 * 1024))
-        gran = num * _ALIGN
-        end = (st.regular_end + gran - 1) // gran * gran
-        if end > st.regular_end:
-            if st.regular_end != st.total:   # irregular tail present: cannot pad in the middle -> shift is not
-                # needed because every offset is _ALIGN aligned; pad only matters at the very end of the range
-                end = st.regular_end // gran * gran
-            else:
-                st.grow(end)
-        offs = sorted((st.offset[p], p) for p in st.order if p not in fz["irregular_params"])
-        tail_regular = [(o, p) for o, p in offs if o >= end]          # regular variables beyond the aligned range
-        offs = [(o, p) for o, p in offs if o < end]
-        if not offs:
+        lay = flat_zero_layout(st, fz, num, self.opt)
+        if lay is None:
+            self._fz_static = None
             return
-        # graded bucket sizes: the variables at the front of the flat buffer belong to the first layers, whose gradients
-        # are produced LAST by the backward pass -- whatever is still in flight when backward ends is exposed, so the
-        # buckets that become ready last are small (4M elements, doubling up to bucket_elems)
-        first = int(self.opt.get("first_bucket_elems", os.environ.get("TEPDIST_FIRST_BUCKET", 4 * 1024 * 1024)))
-        from .. import _C
-        # (the bucket policy lives in the C++ core next to the gradient-collective combiner: csrc/transform.cc PlanFlatBuckets)
-        bounds = list(_C.plan_flat_buckets([int(off) for off, _ in offs], int(end), int(gran), int(first), int(bucket_elems)))
-        buckets = [(bounds[i], bounds[i + 1]) for i in range(len(bounds) - 1)]
-        binding = {k: v for k, v in fz["binding"].items()}
-        regular_apply = set(fz["regular_apply"])
-        skip = set(fz["skip"])
-        if tail_regular:   # (a partially covered variable cannot be split across ownership schemes)
-            cut = {p for _, p in tail_regular}
-            # variables straddling `end` also fall back
-            for o, p in offs:
-                n_el = 1
-                for d in st.shape[p]:
-                    n_el *= d
-                if o + n_el > end:
-                    cut.add(p)
-            if cut:
-                self._fz_static = None
-                return
-        prod_of_param = {pid: key[0] for key, pid in binding.items()}
-        ready_at: Dict[int, List[int]] = {}
-        for bi, (s0, e0) in enumerate(buckets):
-            last = max((prod_of_param[p] for off, p in offs if s0 <= off < e0 and p in prod_of_param), default=-1)
-            ready_at.setdefault(last, []).append(bi)
-        self.grad_binding = binding
-        self.flat_zero = {"level": fz["level"], "num": num, "skip": skip, "buckets": buckets, "ready_at": ready_at,
-                          "rank": self.coords.get(fz["level"], 0), "regular_apply": regular_apply, "fused": None}
+        if lay.total > st.total:
+            st.grow(lay.total)
+        self.grad_binding = dict(fz["binding"])
+        self.flat_zero = {"level": fz["level"], "num": num, "skip": set(fz["skip"]), "layout": lay, "buckets": lay.buckets,
+                          "ready_at": lay.ready_at, "rank": self.coords.get(fz["level"], 0),
+                          "regular_apply": set(fz["regular_apply"]), "fused": None}
         # replicated-gradient variables (e.g. embeddings whose backward the plan replicates on every rank): the gradient
         # lands in the flat buffer and the UPDATE is still sharded -- the owner updates its chunk from the local gradient
         # and publishes it (fused mode: P2P stores from the same kernel; NCCL mode: all-gather).  (N-1)/N less AdamW
         # traffic, and the replicas stay bit-identical (redundant fp32 atomics would let them drift apart).
-        rep = {}
-        if self.opt.get("kind") == "adamw" and st.m is not None:
-            for aid, (pid, gkey) in fz.get("replicated", {}).items():
-                n_el = 1
-                for d in st.shape[pid]:
-                    n_el *= d
-                if n_el % (4 * num) == 0 and st.offset[pid] % 4 == 0 and g.nodes[aid].op == "apply_adamw":
-                    rep[aid] = (pid, st.offset[pid], n_el, bool(g.nodes[aid].attrs.get("decay", True)))
-                    self.grad_binding[gkey] = pid
-        self.flat_zero["replicated_apply"] = rep
+        for aid, (pid, _, _, _) in lay.replicated.items():
+            self.grad_binding[fz["replicated"][aid][1]] = pid
+        self.flat_zero["replicated_apply"] = lay.replicated
         if (self.comm_mode == "fused" and st.master.is_cuda and self.opt.get("kind") == "adamw" and num <= 8):
             from ..parallel.symm import FusedShardedOptimizer
             pg = self.collective.mesh.group(fz["level"])
@@ -582,24 +633,23 @@ class Executor:
             cs = fz["comm_stream"]
             cs.wait_stream(torch.cuda.current_stream())
             s0, e0 = fz["buckets"][bi]
-            n, r = fz["num"], fz["rank"]
-            chunk = (e0 - s0) // n
+            a, b, nd, local = fz["layout"].call(bi, fz["rank"])
             last = len(pending) == len(fz["buckets"]) - 1
             with torch.cuda.stream(cs):
                 if fo.g16 is not None and not fo.dry:      # bf16 wire: stage this bucket's gradients (all of it: peers reduce their chunks of it)
                     ops.cast_f32_bf16(st.grad[s0:e0], fo.g16.tensor(torch.bfloat16, st.total)[s0:e0])
                 fo.barrier()
-                fo.step(st.master, st.m, st.v, s0 + r * chunk, s0 + (r + 1) * chunk, st.n_decay, self.hyper,
+                fo.step(st.master, st.m, st.v, a, b, nd, self.hyper,
                         o.get("beta1", 0.9), o.get("beta2", 0.999), o.get("eps", 1e-8), o.get("weight_decay", 0.0),
-                        ctas=0 if last else int(os.environ.get("TEPDIST_OVERLAP_CTAS", o.get("overlap_ctas", ops._sms() // 2))))   # half the SMs; the rest stay with the backward kernels
+                        ctas=0 if last else int(os.environ.get("TEPDIST_OVERLAP_CTAS", o.get("overlap_ctas", ops._sms() // 2))),   # half the SMs; the rest stay with the backward kernels
+                        local_grad=local)
             pending.append(None)
             return
         s0, e0 = fz["buckets"][bi]
-        n, r = fz["num"], fz["rank"]
-        chunk = (e0 - s0) // n
+        a, b, _, _ = fz["layout"].call(bi, fz["rank"])
         pg = self.collective.mesh.group(fz["level"])
         buf = st.grad[s0:e0]
-        own = st.grad[s0 + r * chunk:s0 + (r + 1) * chunk]
+        own = st.grad[a:b]
         if self.dry_comm:
             pending.append(None)
         elif buf.is_cuda:
@@ -610,7 +660,7 @@ class Executor:
     def _flat_zero_apply(self, pending: List[Any]) -> None:
         import torch.distributed as dist
         fz, st, o = self.flat_zero, self.store, self.opt
-        n, r = fz["num"], fz["rank"]
+        lay, r = fz["layout"], fz["rank"]
         if fz["fused"] is not None:
             fo = fz["fused"]
             cs = fz.get("comm_stream")
@@ -621,11 +671,10 @@ class Executor:
                 if rep:
                     cs.wait_stream(torch.cuda.current_stream())     # their gradients are the last thing backward produces
                 with torch.cuda.stream(cs):
-                    for aid, (pid, off, n_el, decay) in rep.items():
-                        chunk = n_el // n
-                        fo.step(st.master, st.m, st.v, off + r * chunk, off + (r + 1) * chunk, off + n_el if decay else off,
-                                self.hyper, o.get("beta1", 0.9), o.get("beta2", 0.999), o.get("eps", 1e-8),
-                                o.get("weight_decay", 0.0), ctas=0, local_grad=True)
+                    for i in range(lay.n_buckets, len(lay.ranges)):
+                        a, b, nd, local = lay.call(i, r)
+                        fo.step(st.master, st.m, st.v, a, b, nd, self.hyper, o.get("beta1", 0.9), o.get("beta2", 0.999),
+                                o.get("eps", 1e-8), o.get("weight_decay", 0.0), ctas=0, local_grad=local)
                     fo.barrier()    # every rank's parameter shards have landed everywhere
                 torch.cuda.current_stream().wait_stream(cs)
             return
@@ -634,31 +683,19 @@ class Executor:
                 w.wait()
         pg = self.collective.mesh.group(fz["level"])
         works = []
-        for (s0, e0) in fz["buckets"]:
-            chunk = (e0 - s0) // n
-            a, b = s0 + r * chunk, s0 + (r + 1) * chunk
-            nd = min(max(st.n_decay - a, 0), b - a)
-            kind = o.get("kind")
+        kind = o.get("kind")
+        tgt = st.compute if st.compute is not None else st.master
+        for i, (s0, e0, _, _) in enumerate(lay.ranges):     # (the replicated ranges exist for AdamW only)
+            a, b, nd, _ = lay.call(i, r)
             comp = None if st.compute is None else st.compute[a:b]
             if kind == "adamw":
-                ops.adamw_step(st.master[a:b], st.grad[a:b], st.m[a:b], st.v[a:b], comp, nd, self._lr(1e-3),
-                               o.get("beta1", 0.9), o.get("beta2", 0.999), o.get("eps", 1e-8), o.get("weight_decay", 0.0),
-                               self.step_count, hyper=self.hyper if st.master.is_cuda else None)
+                ops.adamw_step(st.master[a:b], st.grad[a:b], st.m[a:b], st.v[a:b], comp, lay.local_decay(a, b, nd),
+                               self._lr(1e-3), o.get("beta1", 0.9), o.get("beta2", 0.999), o.get("eps", 1e-8),
+                               o.get("weight_decay", 0.0), self.step_count, hyper=self.hyper if st.master.is_cuda else None)
             elif kind == "sgd":
                 ops.sgd_step(st.master[a:b], st.grad[a:b], comp, self._lr(1e-2))
-            tgt = st.compute if st.compute is not None else st.master
             if not self.dry_comm:
                 works.append(dist.all_gather_into_tensor(tgt[s0:e0], tgt[a:b], group=pg, async_op=True))
-        for aid, (pid, off, n_el, decay) in (fz.get("replicated_apply") or {}).items():
-            chunk = n_el // n
-            a, b = off + r * chunk, off + (r + 1) * chunk
-            comp = None if st.compute is None else st.compute[a:b]
-            ops.adamw_step(st.master[a:b], st.grad[a:b], st.m[a:b], st.v[a:b], comp, (b - a) if decay else 0, self._lr(1e-3),
-                           o.get("beta1", 0.9), o.get("beta2", 0.999), o.get("eps", 1e-8), o.get("weight_decay", 0.0),
-                           self.step_count, hyper=self.hyper if st.master.is_cuda else None)
-            tgt = st.compute if st.compute is not None else st.master
-            if not self.dry_comm:
-                works.append(dist.all_gather_into_tensor(tgt[off:off + n_el], tgt[a:b], group=pg, async_op=True))
         for w in works:
             w.wait()
 
@@ -671,18 +708,16 @@ class Executor:
             return
         import torch.distributed as dist
         st = self.store
-        n, r = fz["num"], fz["rank"]
+        lay, r = fz["layout"], fz["rank"]
         pg = self.collective.mesh.group(fz["level"])
-        ranges = [(s0, e0) for (s0, e0) in fz["buckets"]]
-        ranges += [(off, off + n_el) for (_, off, n_el, _) in (fz.get("replicated_apply") or {}).values()]
         if st.master.is_cuda:
             torch.cuda.synchronize()
         for buf in (st.master, st.m, st.v):
             if buf is None:
                 continue
-            for (s0, e0) in ranges:
-                chunk = (e0 - s0) // n
-                dist.all_gather_into_tensor(buf[s0:e0], buf[s0 + r * chunk:s0 + (r + 1) * chunk].clone(), group=pg)
+            for i, (s0, e0, _, _) in enumerate(lay.ranges):
+                a, b, _, _ = lay.call(i, r)
+                dist.all_gather_into_tensor(buf[s0:e0], buf[a:b].clone(), group=pg)
 
     # ------------------------------------------------------------------ running
     def step(self, feeds: Dict[str, torch.Tensor]) -> List[torch.Tensor]:
