@@ -20,9 +20,9 @@ one.  Its contiguous halves (chunks 2r, 2r+1) are exchanged into that layout bef
 q / k / v, one for dO / O backward) and the result is exchanged back.  In the zig-zag layout every ring step costs every rank
 the same: the local step is ONE causal product over the rank's block [early; late], a step that holds the block of an
 earlier rank j < r is two half-size unmasked products (both query chunks x the early chunk of j), a later rank's block two
-others (the late query chunk x both chunks of j) -- n/2 block products per rank instead of up to n - 1/2.  CPU-validated
-(gloo, 2 and 4 ranks, against full attention); on GPUs it drives the same block kernels as the contiguous ring but has not
-run there yet, hence opt-in.
+others (the late query chunk x both chunks of j) -- n/2 block products per rank instead of up to n - 1/2.  Validated on
+CPUs (gloo, 2 and 4 ranks, against full attention) and on one GPU (2 and 4 ranks as threads, against fp64 attention); it has
+not run over NCCL between GPUs yet, hence opt-in.
 """
 from __future__ import annotations
 

@@ -1,39 +1,13 @@
-"""GPU numerics of the 128-wide-head attention kernels and of the paths that reach them: padded head widths 65..128, a
-ragged causal sequence, context-parallel ring blocks, GPT-2 with 128-wide heads, and a traced SDPA module.  Every case
-checks that our kernels ran (no torch-math fallback)."""
+"""GPU numerics of the 128-wide-head attention kernels and of the paths that reach them: padded head widths 65..128 and a
+ragged causal sequence (against the fp64 reference of attention_reference.py), GPT-2 with 128-wide heads, and a traced SDPA
+module.  Every case checks that our kernels ran (no torch-math fallback)."""
 import pytest
 import torch
 
+import attention_reference as ar
 import kernel_checks as kc
 
 pytestmark = pytest.mark.gpu
-
-
-def _kernels_only(monkeypatch):
-    """ops, with the torch-math attention paths on CUDA tensors turned into errors (CPU tensors keep the reference)."""
-    from tepdist_b200 import ops
-    from tepdist_b200.ops import attention
-    ref_fwd = attention._ref_fwd
-
-    def fail(*a, **k):
-        raise AssertionError("attention fell back to torch math")
-
-    monkeypatch.setattr(attention, "_ref_fwd", lambda q, *a: fail() if q.is_cuda else ref_fwd(q, *a))
-    monkeypatch.setattr(attention, "_warn_torch_math", fail)
-    ops.lib()
-    return ops
-
-
-def _ref(q, k, v, do, causal):
-    """fp32 autograd attention on [B, S, H, D] -> (o, lse, dq, dk, dv)."""
-    S, D = q.shape[1], q.shape[3]
-    qf, kf, vf = (t.float().detach().clone().requires_grad_(True) for t in (q, k, v))
-    s = torch.einsum("bqhd,bkhd->bhqk", qf, kf) * D ** -0.5
-    if causal:
-        s = s.masked_fill(~torch.ones(S, S, dtype=torch.bool, device=q.device).tril(), float("-inf"))
-    o = torch.einsum("bhqk,bkhd->bqhd", torch.softmax(s, -1), vf)
-    o.backward(do.float())
-    return o.detach(), torch.logsumexp(s, -1).detach(), qf.grad, kf.grad, vf.grad
 
 
 @pytest.mark.parametrize("B,S,H,D,causal", [
@@ -42,7 +16,7 @@ def _ref(q, k, v, do, causal):
     (2, 200, 3, 128, True),                                                  # ragged causal S, padded to 256
 ])
 def test_attention_fwd_bwd_matches_fp32_reference(B, S, H, D, causal, monkeypatch):
-    ops = _kernels_only(monkeypatch)
+    ops = ar.kernels_only(monkeypatch)
     qkv, q, k, v = kc._qkv(B, S, H, D)
     n0 = ops.launch_count()
     o, lse = ops.attention_fwd(q, k, v, causal=causal)
@@ -52,78 +26,14 @@ def test_attention_fwd_bwd_matches_fp32_reference(B, S, H, D, causal, monkeypatc
     ops.attention_bwd(do, q, k, v, o, lse, causal=causal, dqkv_out=buf)
     torch.cuda.synchronize()
     assert ops.launch_count() >= n0 + 7
-    o_ref, lse_ref, *g_ref = _ref(q, k, v, do, causal)
-    assert kc._rel_err(o, o_ref) < 2e-2 and kc._rel_err(lse, lse_ref) < 1e-3
-    for i, want in enumerate(g_ref):
-        assert kc._rel_err(grads[i], want) < 3e-2, i
-        assert kc._rel_err(buf[:, :, :, i], want) < 3e-2, i
-
-
-@pytest.mark.parametrize("n,causal", [(2, True), (2, False), (4, True), (4, False)])
-def test_ring_blocks_hd128(n, causal, monkeypatch):
-    """The serial virtual-rank ring schedule of kernel_checks.check_ring_blocks (causal diagonal block, unmasked blocks through
-    the shared-stride work buffer, log-sum-exp merge, backward blocks fed the global log-sum-exp / output, fp32 accumulation
-    and pack) at D = 128, against full-sequence attention."""
-    ops = _kernels_only(monkeypatch)
-    from tepdist_b200.ops.attention import attn_merge_, attn_ring_accum_, attn_ring_pack
-    B, S, H, D = 2, 512, 2, 128
-    L, dt, dev = S // n, torch.bfloat16, "cuda"
-    qkv, q, k, v = kc._qkv(B, S, H, D, seed=3)
-    do = torch.randn(B, S, H, D, device=dev).to(dt)
-    o_ref, lse_ref, *g_ref = _ref(q, k, v, do, causal)
-    blk = lambda t, r: t[:, r * L:(r + 1) * L]
-    o_all = torch.empty(B, S, H, D, device=dev, dtype=dt)
-    lse_all = torch.empty(B, H, S, device=dev)
-    dq_acc = torch.zeros(n, B, L, H, D, device=dev)
-    kv_acc = torch.zeros(n, B, L, H, 2, D, device=dev)
-    n0 = ops.launch_count()
-    for r in range(n):
-        o_acc = torch.empty(B, L, H, D, device=dev)
-        la, lb = torch.empty(B, H, L, device=dev), torch.empty(B, H, L, device=dev)
-        work = torch.empty(B, L, H, 3, D, device=dev, dtype=dt)
-        work[:, :, :, 0].copy_(blk(q, r))
-        first = True
-        for t in range(n):
-            j = (r - t) % n
-            if causal and j > r:
-                continue
-            if t == 0:
-                o_j, lse_j = ops.attention_fwd(blk(q, r), blk(k, r), blk(v, r), causal=causal)
-            else:
-                work[:, :, :, 1:].copy_(torch.stack((blk(k, j), blk(v, j)), 3))
-                o_j, lse_j = ops.attention_fwd(work[:, :, :, 0], work[:, :, :, 1], work[:, :, :, 2], causal=False)
-            attn_merge_(o_acc, la, lb, o_j.contiguous(), lse_j.contiguous(), first)
-            la, lb, first = lb, la, False
-        blk(o_all, r).copy_(o_acc)
-        lse_all[:, :, r * L:(r + 1) * L].copy_(la)
-    for r in range(n):
-        work = torch.empty(B, L, H, 3, D, device=dev, dtype=dt)
-        work[:, :, :, 0].copy_(blk(q, r))
-        part = torch.empty(B, L, H, 3, D, device=dev, dtype=dt)
-        o_r, lse_r, do_r = blk(o_all, r).contiguous(), lse_all[:, :, r * L:(r + 1) * L].contiguous(), blk(do, r).contiguous()
-        for t in range(n):
-            j = (r - t) % n
-            if causal and j > r:
-                continue
-            if t == 0:
-                ops.attention_bwd(do_r, blk(q, r), blk(k, r), blk(v, r), o_r, lse_r, causal=causal, dqkv_out=part)
-            else:
-                work[:, :, :, 1:].copy_(torch.stack((blk(k, j), blk(v, j)), 3))
-                ops.attention_bwd(do_r, work[:, :, :, 0], work[:, :, :, 1], work[:, :, :, 2], o_r, lse_r, causal=False, dqkv_out=part)
-            attn_ring_accum_(dq_acc[r], kv_acc[j], part)
-    g = torch.empty(B, S, H, 3, D, device=dev, dtype=dt)
-    for r in range(n):
-        blk(g, r).copy_(attn_ring_pack(dq_acc[r], kv_acc[r], torch.empty(B, L, H, 3, D, device=dev, dtype=dt)))
-    torch.cuda.synchronize()
-    assert ops.launch_count() > n0
-    assert kc._rel_err(o_all, o_ref) < 3e-2 and kc._rel_err(lse_all, lse_ref) < 3e-2
-    for i, want in enumerate(g_ref):
-        assert kc._rel_err(g[:, :, :, i], want) < 3e-2, i
+    ref = ar.reference(q, k, v, do, causal)
+    ref.check(o=o, lse=lse, dq=grads[0], dk=grads[1], dv=grads[2])
+    ref.check(dq=buf[:, :, :, 0], dk=buf[:, :, :, 1], dv=buf[:, :, :, 2])
 
 
 def test_hd128_long_sequence_memory_stays_linear(monkeypatch):
     """S = 8192: one fp32 [H, S, S] score tensor alone would be 2 GB; the kernels need no S x S storage."""
-    ops = _kernels_only(monkeypatch)
+    ops = ar.kernels_only(monkeypatch)
     B, S, H, D = 1, 8192, 8, 128
     qkv, q, k, v = kc._qkv(B, S, H, D)
     do = torch.randn(B, S, H, D, device="cuda", dtype=torch.bfloat16)
@@ -140,7 +50,7 @@ def test_hd128_long_sequence_memory_stays_linear(monkeypatch):
 
 
 def test_gpt2_hd128_trains_and_matches_cpu_reference(monkeypatch):
-    _kernels_only(monkeypatch)
+    ar.kernels_only(monkeypatch)
     from tepdist_b200.models.gpt2 import CONFIGS, build_gpt2_graph
     from tepdist_b200.runtime.executor import Executor
     cfg = CONFIGS["tiny-hd128"]
@@ -198,7 +108,7 @@ def test_traced_sdpa_block_with_128_wide_heads(monkeypatch):
                compute_dtype="bf16")
     assert any(n.op == "attention" for n in tr.graph.nodes)
     net = net.cuda()
-    ops = _kernels_only(monkeypatch)
+    ops = ar.kernels_only(monkeypatch)
     ex = Executor(tr.graph, torch.device("cuda", 0), use_cuda_graph=False)
     tr.load_state_dict_into(ex, net.state_dict())
     opt = torch.optim.SGD(net.parameters(), lr=0.1)

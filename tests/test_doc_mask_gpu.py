@@ -1,29 +1,16 @@
 """GPU numerics of document-masked causal attention and per-document positions (packed rows): the doc_starts kernel, the
-DOC instantiations of the flash forward / backward at D = 64 / 128 (and padded 32 / 80, ragged S) against an fp64 reference,
-the per-document embedding, and whole GPT-2 steps against the CPU executor.  Every case checks that our kernels ran: the
-launch counter grows and the torch-math attention paths are turned into errors."""
+DOC instantiations of the flash forward / backward at D = 64 / 128 (and padded 32 / 80, ragged S) against the fp64 reference
+of attention_reference.py, the per-document embedding, and whole GPT-2 steps against the CPU executor.  Every case checks
+that our kernels ran: the launch counter grows and the torch-math attention paths are turned into errors."""
 import pytest
 import torch
 
+import attention_reference as ar
 import kernel_checks as kc
 
 pytestmark = pytest.mark.gpu
 
 EOT = 999
-
-
-def _kernels_only(monkeypatch):
-    from tepdist_b200 import ops
-    from tepdist_b200.ops import attention
-    ref_fwd = attention._ref_fwd
-
-    def fail(*a, **k):
-        raise AssertionError("attention fell back to torch math")
-
-    monkeypatch.setattr(attention, "_ref_fwd", lambda q, *a: fail() if q.is_cuda else ref_fwd(q, *a))
-    monkeypatch.setattr(attention, "_warn_torch_math", fail)
-    ops.lib()
-    return ops
 
 
 def _tokens(layout: str, B: int, S: int) -> torch.Tensor:
@@ -44,32 +31,11 @@ def _tokens(layout: str, B: int, S: int) -> torch.Tensor:
     return tok.cuda()
 
 
-def _ref64(q, k, v, do, ds):
-    """fp64 autograd attention on [B, S, H, D] with the document mask -> (o, lse, dq, dk, dv)."""
-    S, D = q.shape[1], q.shape[3]
-    qf, kf, vf = (t.double().detach().clone().requires_grad_(True) for t in (q, k, v))
-    s = torch.einsum("bqhd,bkhd->bhqk", qf, kf) * D ** -0.5
-    keys = torch.arange(S, device=q.device)
-    mask = torch.ones(S, S, dtype=torch.bool, device=q.device).tril() & (keys.view(1, 1, S) >= ds.long().unsqueeze(-1)).unsqueeze(1)
-    s = s.masked_fill(~mask, float("-inf"))
-    o = torch.einsum("bhqk,bkhd->bqhd", torch.softmax(s, -1), vf)
-    o.backward(do.double())
-    return o.detach(), torch.logsumexp(s, -1).detach(), qf.grad, kf.grad, vf.grad
-
-
-def _close(got, want, rel, what):
-    got = got.double()
-    assert torch.isfinite(got).all(), f"{what}: non-finite values"
-    assert kc._rel_err(got, want) < rel, (what, kc._rel_err(got, want))
-    err = (got - want).abs().max().item()
-    assert err <= 4 * rel * want.abs().max().item() + 1e-3, (what, err, want.abs().max().item())
-
-
 @pytest.mark.parametrize("S", [128, 1000, 1024, 4096])
 @pytest.mark.parametrize("D", [64, 128, 32, 80])
 @pytest.mark.parametrize("layout", ["len1", "on_boundary", "before_boundary", "nan_tile", "many_short"])
 def test_doc_masked_attention_matches_fp64_reference(layout, D, S, monkeypatch):
-    ops = _kernels_only(monkeypatch)
+    ops = ar.kernels_only(monkeypatch)
     B, H = 2, 2
     ds = ops.doc_starts(_tokens(layout, B, S), EOT)
     qkv, q, k, v = kc._qkv(B, S, H, D, seed=S + D)
@@ -79,16 +45,12 @@ def test_doc_masked_attention_matches_fp64_reference(layout, D, S, monkeypatch):
     dq, dk, dv = ops.attention_bwd(do, q, k, v, o, lse, causal=True, doc_start=ds)
     torch.cuda.synchronize()
     assert ops.launch_count() >= n0 + 4
-    o_ref, lse_ref, *g_ref = _ref64(q, k, v, do, ds)
-    _close(o, o_ref, 2e-2, "o")
-    _close(lse, lse_ref, 1e-3, "lse")
-    for name, got, want in zip(("dq", "dk", "dv"), (dq, dk, dv), g_ref):
-        _close(got, want, 3e-2, name)
+    ar.reference(q, k, v, do, True, ds).check(o=o, lse=lse, dq=dq, dk=dk, dv=dv)
 
 
 @pytest.mark.parametrize("S", [1, 255, 256, 257, 1000, 4096])
 def test_doc_starts_kernel_matches_reference(S, monkeypatch):
-    ops = _kernels_only(monkeypatch)
+    ops = ar.kernels_only(monkeypatch)
     g = torch.Generator().manual_seed(S)
     tok = torch.randint(0, 20, (3, S), generator=g, dtype=torch.int32)
     tok[1] = EOT   # consecutive EOTs everywhere
@@ -106,7 +68,7 @@ def test_all_zero_doc_start_equals_plain_causal_kernel(D, S, monkeypatch):
     """With every document start at 0 the DOC kernels do the plain kernels' arithmetic in the same order.  O, lse, dK and dV
     are bit-identical; dQ is summed over KV blocks with fp32 atomics, whose order differs between any two runs (of the plain
     kernel too), so it is compared to rounding."""
-    ops = _kernels_only(monkeypatch)
+    ops = ar.kernels_only(monkeypatch)
     B, H = 2, 4
     qkv, q, k, v = kc._qkv(B, S, H, D, seed=11)
     do = torch.randn(B, S, H, D, device="cuda").to(torch.bfloat16)
@@ -122,7 +84,7 @@ def test_all_zero_doc_start_equals_plain_causal_kernel(D, S, monkeypatch):
 
 
 def test_per_document_embedding_is_exact(monkeypatch):
-    ops = _kernels_only(monkeypatch)
+    ops = ar.kernels_only(monkeypatch)
     B, S, C, V = 3, 1024, 256, 1000
     tok = _tokens("many_short", B, S)
     ds = ops.doc_starts(tok, EOT)
@@ -147,7 +109,7 @@ def test_per_document_embedding_is_exact(monkeypatch):
 
 @pytest.mark.parametrize("name", ["tiny", "tiny-hd128"])
 def test_gpt2_with_documents_trains_and_matches_cpu_reference(name, monkeypatch):
-    ops = _kernels_only(monkeypatch)
+    ops = ar.kernels_only(monkeypatch)
     from tepdist_b200.models.gpt2 import CONFIGS, build_gpt2_graph
     from tepdist_b200.runtime.executor import Executor
     cfg = CONFIGS[name]

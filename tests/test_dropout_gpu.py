@@ -1,13 +1,16 @@
 """Dropout on the H100 (DESIGN.md "Dropout"): the kernels' masks equal the host mask bit for bit (the elementwise kernel on
 ones; the attention kernels read back through O with uniform probabilities and a one-hot V), attention forward / backward
-with dropout against an fp64 reference that uses the host mask, whole GPT-2 steps with all three dropouts against the fp32
-CPU executor, and CUDA-graph replay (the step is read from device memory, not frozen into the graph)."""
+with dropout against the fp64 reference of attention_reference.py with the host mask, whole GPT-2 steps with all three
+dropouts against the fp32 CPU executor, and CUDA-graph replay (the step is read from device memory, not frozen into the
+graph)."""
 import math
 import os
 import sys
 
 import pytest
 import torch
+
+import attention_reference as ar
 
 pytestmark = pytest.mark.gpu
 
@@ -17,18 +20,13 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 @pytest.fixture
 def ops(monkeypatch):
     """The kernel layer; torch-math attention and torch-fallback warnings are failures."""
-    from tepdist_b200 import ops as _ops
-    from tepdist_b200.ops import attention
-    _ops.lib()
-    ref_fwd = attention._ref_fwd
+    ops_ = ar.kernels_only(monkeypatch)
 
     def fail(*a, **k):
         raise AssertionError("fell back to torch math instead of our kernel")
 
-    monkeypatch.setattr(attention, "_ref_fwd", lambda q, *a, **k: fail() if q.is_cuda else ref_fwd(q, *a, **k))
-    monkeypatch.setattr(attention, "_warn_torch_math", fail)
-    monkeypatch.setattr(_ops, "_warn_once", fail)
-    return _ops
+    monkeypatch.setattr(ops_, "_warn_once", fail)
+    return ops_
 
 
 def _state(step, micro=0):
@@ -107,31 +105,6 @@ def test_attention_kernel_mask_equals_host_mask(ops, B, S, H, D, causal, doc, b_
 
 
 # ------------------------------------------------------------------ numerics against fp64
-def _ref(q, k, v, do, causal, z, doc=None):
-    """fp64 autograd attention with the scaled keep mask z [B, H, S, S] on the probabilities -> (o, lse, dq, dk, dv)."""
-    S, D = q.shape[1], q.shape[3]
-    qf, kf, vf = (t.double().detach().clone().requires_grad_(True) for t in (q, k, v))
-    s = torch.einsum("bqhd,bkhd->bhqk", qf, kf) * D ** -0.5
-    if causal:
-        vis = torch.ones(S, S, dtype=torch.bool, device=q.device).tril()
-        if doc is not None:
-            vis = vis & (torch.arange(S, device=q.device).view(1, 1, S) >= doc.long().unsqueeze(-1)).unsqueeze(1)
-        s = s.masked_fill(~vis, float("-inf"))
-    o = torch.einsum("bhqk,bkhd->bqhd", torch.softmax(s, -1) * z, vf)
-    o.backward(do.double())
-    return o.detach(), torch.logsumexp(s, -1).detach(), qf.grad, kf.grad, vf.grad
-
-
-def _close(got, want, rel, what):
-    """As test_attention_hd64_gpu.py: norm-relative error under `rel`, every element within 4 rel of the largest magnitude."""
-    got = got.double()
-    assert torch.isfinite(got).all(), f"{what}: non-finite values"
-    err_norm = ((got - want).norm() / (want.norm() + 1e-12)).item()
-    assert err_norm < rel, (what, err_norm)
-    err = (got - want).abs().max().item()
-    assert err <= 4 * rel * want.abs().max().item() + 1e-3, (what, err, want.abs().max().item())
-
-
 NUM_CASES = [   # (B, S, H, D, causal, doc): the 345M and 1.3B step shapes
     (4, 1024, 16, 64, True, False),
     (4, 1024, 16, 64, False, False),
@@ -163,12 +136,9 @@ def test_attention_with_dropout_matches_fp64(ops, B, S, H, D, causal, doc):
     torch.cuda.synchronize()
     assert ops.launch_count() >= n0 + 4
     z = keep_mask(rng, p, B, H, S, D).cuda().double() * (256.0 / (256 - ops.dropout_threshold(p)))
-    o_ref, lse_ref, *g_ref = _ref(q, k, v, do, causal, z, ds)
+    ref = ar.reference(q, k, v, do, causal, ds, z)
     del z
-    _close(o, o_ref, 2e-2, "o")
-    _close(lse, lse_ref, 1e-3, "lse")
-    for name, got, want in zip(("dq", "dk", "dv"), (dq, dk, dv), g_ref):
-        _close(got, want, 3e-2, name)
+    ref.check(o=o, lse=lse, dq=dq, dk=dk, dv=dv)
 
 
 # ------------------------------------------------------------------ whole steps
