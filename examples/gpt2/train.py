@@ -5,6 +5,7 @@ loader (tepdist_b200/data: memory-mapped uint16 / int32 token streams, windows o
 `--data synthetic` for a fresh random batch every step from the same loader."""
 import argparse
 import dataclasses
+import math
 import os
 import sys
 import time
@@ -38,6 +39,10 @@ def main():
                     help="end-of-text token id (50256 for GPT-2): attention stays inside each packed document")
     ap.add_argument("--reset-position-ids", action="store_true",
                     help="learned positions count from each document's start (needs --eot-token)")
+    ap.add_argument("--eval-data", default=None,
+                    help="held-out token files (comma-separated) or 'synthetic': evaluation loss and perplexity, dropout off")
+    ap.add_argument("--eval-every", type=int, default=0, help="evaluate after every N training steps (0: never)")
+    ap.add_argument("--eval-batches", type=int, default=4, help="batches per evaluation")
     a = ap.parse_args()
     clip = {"clip_norm": a.clip_norm, "clip_norm_value": a.clip_norm_value} if a.clip_norm else {}
     cfg = CONFIGS[a.model]
@@ -61,11 +66,26 @@ def main():
         tok = torch.randint(0, cfg.n_vocab, (a.batch * world, cfg.n_ctx), generator=gen, dtype=torch.int32)
         fixed = {"tokens": tok, "labels": torch.roll(tok, -1, 1)}
         batches = iter(lambda: fixed, None)
+    eval_batches = None
+    if a.eval_data and a.eval_every > 0:
+        # its own fixed seed and step 0 on every evaluation: every evaluation sees the same held-out batches
+        from tepdist_b200.data import TokenLoader
+        src = ({"synthetic_vocab": cfg.n_vocab} if a.eval_data == "synthetic" else
+               {"files": a.eval_data.split(","), "bytes_per_token": 4 if a.data_int32 else 2})
+        eval_batches = [{k: v.clone() for k, v in b.items()} for b, _ in zip(TokenLoader(batch=a.batch * world, n_ctx=cfg.n_ctx, seed=a.seed + 1_000_003, start_step=0,
+                                                      **src), range(a.eval_batches))]
     t0 = time.time()
     for i in range(a.train_steps):
         loss = tr.step(next(batches))
         if tr.rank == 0:
             print(f"step {i} loss {loss:.4f}")
+        if eval_batches and (i + 1) % a.eval_every == 0:
+            total, tokens = 0.0, 0
+            for b in eval_batches:
+                s, n = tr.evaluate(b)
+                total, tokens = total + s, tokens + n
+            if tr.rank == 0:
+                print(f"step {i} eval loss {total / tokens:.4f} ppl {math.exp(total / tokens):.2f} ({tokens} tokens)")
     if tr.rank == 0:
         dt = time.time() - t0
         print(f"Train loop took {dt:.2f} s  ({a.train_steps * a.batch * world * cfg.n_ctx / dt:.0f} tokens/s incl. planning + warm-up); "

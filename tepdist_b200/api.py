@@ -12,7 +12,7 @@ Launch with torchrun (one process per GPU); single-process works for 1 GPU / CPU
 from __future__ import annotations
 
 import os
-from typing import Any, Dict, Optional
+from typing import Any, Dict, Optional, Tuple
 
 import torch
 import torch.distributed as dist
@@ -92,6 +92,23 @@ class Trainer:
     def step_async(self, dev_feeds: Dict[str, torch.Tensor]) -> torch.Tensor:
         """Device-resident variant (no host sync): returns the loss tensor."""
         return self.exec.step(dev_feeds)[0]
+
+    def evaluate(self, feeds: Dict[str, torch.Tensor]) -> Tuple[float, int]:
+        """Validation loss of one batch: dropout off, forward only, nothing of the training state changes.  Returns
+        (loss_sum, tokens) over the GLOBAL batch, the same on every rank; labels < 0 are ignored (padding), so
+        loss_sum / tokens is the mean over the real tokens and exp of it the perplexity.  Raises ValueError if a label is
+        >= the vocabulary size.  Host tensors are copied to the device as in `step` (never from the FAKE_INPUT cache)."""
+        dev_feeds = {k: t if t.device == self.device else t.to(self.device, non_blocking=True) for k, t in feeds.items()}
+        s, n, bad = (float(x) for x in self.evaluate_async(dev_feeds).cpu())
+        if bad:
+            raise ValueError(f"evaluate: {int(bad)} label(s) >= the vocabulary size")
+        return s, int(n)
+
+    def evaluate_async(self, dev_feeds: Dict[str, torch.Tensor]) -> torch.Tensor:
+        """Device-resident variant of `evaluate` (no host sync): fp64 [3] = (loss_sum, tokens, labels >= vocab).  A tensor of
+        its own (a copy of the captured evaluation's output buffer, which the next evaluation overwrites), so triples of
+        several batches can be summed without a sync."""
+        return self.exec.evaluate(dev_feeds).clone()
 
     def executor(self):
         """The Executor that owns this rank's variables: the whole (sharded) step graph, or -- under a pipeline plan -- this

@@ -126,6 +126,15 @@ struct Rewriter {
       const TensorType& l = g.type(n.inputs[0]);
       int64_t tokens = n.has("global_tokens") ? n.attr_i("global_tokens") : l.numel() / l.dims.back();
       a["global_tokens"] = tokens;
+      if (c.ins[0].is_split()) {
+        // the tokens are split over this level (the loss has no vocab candidate): an evaluation step sums its (loss, token
+        // count) over exactly the levels recorded here
+        std::vector<int64_t> lv = n.attr_v("token_levels"), nm = n.attr_v("token_nums");
+        lv.push_back((int64_t)level);
+        nm.push_back((int64_t)num);
+        a["token_levels"] = lv;
+        a["token_nums"] = nm;
+      }
     }
     if (op == "reduce_mean" && c.outs[0].partial) {
       const TensorType& x = g.type(n.inputs[0]);

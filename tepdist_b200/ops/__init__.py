@@ -95,6 +95,8 @@ class _Sig:
     tepd_embedding_bwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]
     tepd_doc_starts = [_vp, _vp, _i, _i, _i, _vp]
     tepd_xent_fwd_bwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp]
+    tepd_xent_fwd = [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]
+    tepd_gemm_last_epi = []
     tepd_adamw = [_vp, _vp, _vp, _vp, _vp, _ll, _ll, _f, _f, _f, _f, _f, _f, _f, _f, _vp, _vp]
     tepd_sgd = [_vp, _vp, _vp, _ll, _f, _f, _vp]
     tepd_optim_step = [_i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
@@ -148,7 +150,8 @@ def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn: bool = False, b_mn: bool = F
     Storage: ``a`` is [.., M, K] (a_mn=False) or [.., K, M] (a_mn=True); ``b`` is [.., N, K]
     (b_mn=False, i.e. nn.Linear weight layout) or [.., K, N] (b_mn=True).  Optional leading batch dim.
     ``accumulate`` adds into an fp32 ``out`` (gradient accumulation / split-K reduction target).
-    ``act="gelu"`` with ``out2``: ``out`` receives the pre-activation, ``out2`` the activated value (one pass).
+    ``act="gelu"`` with ``out2``: ``out`` receives the pre-activation, ``out2`` the activated value (one pass); without
+    ``out2``, ``out`` receives the activated value only.
     ``act="gelu_bwd"`` with ``aux`` (pre-activation): the result is multiplied by GELU'(aux) in the epilogue.
     ``split_k``: 0 = automatic, 1 = one unit per output tile, s > 1 = split-K over s units, -1 = stream-K.  Split-K and
     stream-K units add their partials into ``out``, so they need ``accumulate`` with an fp32 ``out``.
@@ -779,6 +782,30 @@ def xent_fwd_bwd(logits: torch.Tensor, labels: torch.Tensor, vocab: int, grad_sc
                                    grad_scale, _stream()), "xent_fwd_bwd")
     _count()
     return total, rows
+
+
+def xent_fwd(logits: torch.Tensor, labels: torch.Tensor, vocab: int):
+    """Forward-only softmax-cross-entropy for evaluation: ``logits`` [T, Vp] is read once and not written.  Labels < 0 are
+    ignored and labels >= vocab are counted as bad; neither contributes a loss.  Returns (fp64 [3] = (loss sum over the
+    valid labels, number of valid labels, number of bad labels), per-row fp32 loss with 0 on ignored and bad rows).  The
+    sum runs in a fixed order, so repeated calls give the same bits."""
+    T, Vp = logits.shape
+    if not logits.is_cuda:
+        lab = labels.long().reshape(-1)
+        valid = (lab >= 0) & (lab < vocab)
+        lf = logits.float()[:, :vocab]
+        rows = torch.logsumexp(lf, -1) - lf.gather(1, torch.where(valid, lab, 0).unsqueeze(1)).squeeze(1)
+        rows = torch.where(valid, rows, torch.zeros_like(rows))
+        out = torch.stack([rows.double().sum(), valid.sum().double(), (lab >= vocab).sum().double()])
+        return out, rows
+    assert logits.is_contiguous() and logits.dtype == torch.bfloat16
+    lab = labels.to(torch.int32).contiguous()
+    rows = torch.empty(T, dtype=torch.float32, device=logits.device)
+    out = torch.empty(3, dtype=torch.float64, device=logits.device)
+    _check(lib().tepd_xent_fwd(logits.data_ptr(), lab.data_ptr(), rows.data_ptr(), out.data_ptr(), T, vocab, Vp, _stream()),
+           "xent_fwd")
+    _count(2)
+    return out, rows
 
 
 # --------------------------------------------------------------------------------------------- optimizer

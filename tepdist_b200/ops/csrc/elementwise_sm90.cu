@@ -533,6 +533,97 @@ __global__ void __launch_bounds__(512) xent_fwd_bwd_kernel(bf16* __restrict__ lo
   }
 }
 
+// ------------------------------------------------------------------ softmax cross-entropy, forward only (evaluation)
+// One block per row, ONE read of the row: every thread keeps a running (max, sum of exp(x - max)) over its 8-element vectors
+// (columns >= V do not take part), the block merges the pairs.  The logits are never written.  The row loss is
+// log(sum) + max - logit[label]; rows whose label is < 0 (ignored) or >= V (bad) get 0.  Four vectors are loaded before any
+// is used, so each thread has 64 bytes in flight.
+__device__ __forceinline__ void lse_merge(float& m, float& s, float m2, float s2) {
+  const float mm = fmaxf(m, m2);
+  if (mm == -INFINITY) return;   // both empty
+  s = s * __expf(m - mm) + s2 * __expf(m2 - mm);
+  m = mm;
+}
+__global__ void __launch_bounds__(512) xent_fwd_kernel(const bf16* __restrict__ logits, const int* __restrict__ labels,
+                                                      float* __restrict__ loss_rows, int V, int Vp) {
+  __shared__ float sm[16], ss[16];
+  const int row = blockIdx.x;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint4* lr = reinterpret_cast<const uint4*>(logits + (size_t)row * Vp);
+  const int nvec = (V + 7) >> 3;    // vectors holding a column < V (V <= Vp, Vp % 8 == 0)
+  float m = -INFINITY, s = 0.f;
+  for (int i0 = threadIdx.x; i0 < nvec; i0 += 4 * 512) {
+    uint4 u[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (i0 + k * 512 < nvec) u[k] = __ldcs(lr + i0 + k * 512);   // streamed: each row is read once
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int i = i0 + k * 512;
+      if (i >= nvec) break;
+      float f[8];
+      unpack8(u[k], f);
+      float mv = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (i * 8 + j < V) mv = fmaxf(mv, f[j]);
+      if (mv == -INFINITY) continue;   // adds nothing; with m = -inf too, exp(x - m) would be exp(-inf + inf) = NaN
+      if (mv > m) { s *= __expf(m - mv); m = mv; }
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (i * 8 + j < V) s += __expf(f[j] - m);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+    lse_merge(m, s, m2, s2);
+  }
+  if (lane == 0) { sm[warp] = m; ss[warp] = s; }
+  __syncthreads();
+  if (warp == 0) {
+    m = lane < 16 ? sm[lane] : -INFINITY;
+    s = lane < 16 ? ss[lane] : 0.f;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+      lse_merge(m, s, m2, s2);
+    }
+    if (lane == 0) {
+      const int lab = labels[row];
+      float l = 0.f;
+      if (lab >= 0 && lab < V) l = __logf(s) + m - __bfloat162float(logits[(size_t)row * Vp + lab]);
+      loss_rows[row] = l;
+    }
+  }
+}
+
+// (loss_sum, valid_tokens, bad_labels) of one batch in fp64, always in the same order: thread t sums rows t, t + 1024, ...,
+// then a fixed shared-memory tree.  Repeated calls and graph replays give the same bits.
+__global__ void __launch_bounds__(1024) xent_sum_kernel(const float* __restrict__ loss_rows, const int* __restrict__ labels,
+                                                       double* __restrict__ out, int T, int V) {
+  __shared__ double s_sum[1024];
+  __shared__ int s_valid[1024], s_bad[1024];
+  double sum = 0.0;
+  int valid = 0, bad = 0;
+  for (int r = threadIdx.x; r < T; r += 1024) {
+    const int lab = labels[r];
+    if (lab >= V) ++bad;
+    else if (lab >= 0) { ++valid; sum += (double)loss_rows[r]; }
+  }
+  s_sum[threadIdx.x] = sum; s_valid[threadIdx.x] = valid; s_bad[threadIdx.x] = bad;
+  __syncthreads();
+  for (int w = 512; w > 0; w >>= 1) {
+    if (threadIdx.x < w) {
+      s_sum[threadIdx.x] += s_sum[threadIdx.x + w];
+      s_valid[threadIdx.x] += s_valid[threadIdx.x + w];
+      s_bad[threadIdx.x] += s_bad[threadIdx.x + w];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) { out[0] = s_sum[0]; out[1] = (double)s_valid[0]; out[2] = (double)s_bad[0]; }
+}
+
 // ------------------------------------------------------------------ fused AdamW over flat buffers
 // master fp32 params, fp32 grads (already summed/averaged), fp32 m/v; writes the bf16 compute copy.
 // wd_mask: per-"segment" weight decay is encoded by the caller splitting the flat buffer into a decayed
@@ -803,6 +894,14 @@ extern "C" int tepd_xent_fwd_bwd(void* logits, const void* labels, void* loss_ro
                                  float gscale, void* stream) {
   if (Vp % 8) return -2;
   xent_fwd_bwd_kernel<<<T, 512, 0, CS(stream)>>>((bf16*)logits, (const int*)labels, (float*)loss_rows, (float*)loss_sum, V, Vp, gscale);
+  return (int)cudaGetLastError();
+}
+// out: fp64 [3] = (sum of the row losses of labels in [0, V), number of such labels, number of labels >= V)
+extern "C" int tepd_xent_fwd(const void* logits, const void* labels, void* loss_rows, void* out, int T, int V, int Vp,
+                             void* stream) {
+  if (Vp % 8 || V <= 0 || V > Vp || T <= 0) return -2;
+  xent_fwd_kernel<<<T, 512, 0, CS(stream)>>>((const bf16*)logits, (const int*)labels, (float*)loss_rows, V, Vp);
+  xent_sum_kernel<<<1, 1024, 0, CS(stream)>>>((const float*)loss_rows, (const int*)labels, (double*)out, T, V);
   return (int)cudaGetLastError();
 }
 extern "C" int tepd_adamw(void* p, const void* g, void* m, void* v, void* p_bf16, long long n, long long n_decay, float lr,

@@ -118,8 +118,11 @@ enum Epi : int {
   EPI_GELU_BWD,    // alpha * acc * GELU'(aux)
   EPI_F32,         // fp32 D = alpha * acc
   EPI_F32_ADD,     // fp32 D += alpha * acc (TMA reduce-add: split-K, stream-K and gradient accumulation)
+  EPI_BIAS_GELU,   // D = GELU(alpha * acc + bias), no pre-activation output (forward-only MLP)
 };
-template <int EPI> __host__ __device__ constexpr bool epi_bias() { return EPI == EPI_BIAS || EPI == EPI_BIAS_RES || EPI == EPI_GELU_DUAL; }
+template <int EPI> __host__ __device__ constexpr bool epi_bias() {
+  return EPI == EPI_BIAS || EPI == EPI_BIAS_RES || EPI == EPI_GELU_DUAL || EPI == EPI_BIAS_GELU;
+}
 template <int EPI> __host__ __device__ constexpr bool epi_tile_in() { return EPI == EPI_BIAS_RES || EPI == EPI_GELU_BWD; }
 template <int EPI> __host__ __device__ constexpr bool epi_f32() { return EPI == EPI_F32 || EPI == EPI_F32_ADD; }
 
@@ -394,6 +397,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUten
                   if constexpr (EPI == EPI_GELU_DUAL) {
                     if (r == 1) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
                   }
+                  if constexpr (EPI == EPI_BIAS_GELU) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
                   if constexpr (epi_tile_in<EPI>()) {
                     uint32_t in;
                     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(in) : "r"(addr));
@@ -522,6 +526,10 @@ static int launch_gemm(const Maps& m, const GemmParams& p, int num_sms, cudaStre
   return (int)tepd::launch(kern, dim3(grid), dim3(NUM_THREADS), C::SMEM_BYTES, stream, m.a, m.b, m.d, m.d2, m.in, p);
 }
 
+// Epilogue kind of this thread's last tepd_gemm_bf16 call (an Epi value), so tests can tell which path ran.
+static thread_local int g_last_epi = -1;
+extern "C" int tepd_gemm_last_epi() { return g_last_epi; }
+
 // C ABI entry (called from Python via ctypes).  All leading dims / strides are in elements.
 extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void* bias, const void* residual,
                               int M, int N, int K, int batch, long long lda, long long ldb, long long ldd,
@@ -574,7 +582,8 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
   if (rc) return 200 + rc;
   // Epilogue kind.  bf16 outputs go through shared memory and TMA when TMA can address the output and the residual / aux
   // (16-byte aligned base, row pitch and batch stride; aux and D2 share D's layout) and a staged kind exists for the
-  // flags and the operand layout: plain for every layout, bias / bias + residual / dual GELU for the forward layout
+  // flags and the operand layout: plain for every layout, bias / bias + residual / dual GELU / single-output GELU for the
+  // forward layout
   // (A and B K-major), GELU' for the data-gradient layout (B MN-major).  fp32 outputs of the weight-gradient layout (A and B
   // MN-major) without bias, residual or activation go through shared memory too: plain stores, or TMA reduce-adds for
   // accumulating outputs (split-K, stream-K, gradient accumulation).  Everything else stores from the fragments.
@@ -587,10 +596,12 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
     else if (act == 0 && !residual && fwd) epi = EPI_BIAS;
     else if (act == 0 && res_ok && fwd) epi = EPI_BIAS_RES;
     else if (act == 1 && D2 && al16(D2) && !residual && fwd) epi = EPI_GELU_DUAL;
+    else if (act == 1 && !D2 && !residual && fwd) epi = EPI_BIAS_GELU;
     else if (act == 2 && al16(aux) && !bias && !residual && dgrad) epi = EPI_GELU_BWD;
   }
   if (out_fp32 && wgrad && act == 0 && !bias && !residual && ldd % 4 == 0 && (batch == 1 || stride_d % 4 == 0) && al16(D))
     epi = accumulate ? EPI_F32_ADD : EPI_F32;
+  g_last_epi = epi;
   Maps m;
   m.a = ta; m.b = tb;
   m.d = m.d2 = m.in = CUtensorMap{};
@@ -616,6 +627,7 @@ extern "C" int tepd_gemm_bf16(const void* A, const void* B, void* D, const void*
     case EPI_BIAS: return launch_gemm<BN, false, false, EPI_BIAS>(m, p, num_sms, s);               \
     case EPI_BIAS_RES: return launch_gemm<BN, false, false, EPI_BIAS_RES>(m, p, num_sms, s);       \
     case EPI_GELU_DUAL: return launch_gemm<BN, false, false, EPI_GELU_DUAL>(m, p, num_sms, s);     \
+    case EPI_BIAS_GELU: return launch_gemm<BN, false, false, EPI_BIAS_GELU>(m, p, num_sms, s);     \
     case EPI_GELU_BWD: return launch_gemm<BN, false, true, EPI_GELU_BWD>(m, p, num_sms, s);        \
     case EPI_F32: return launch_gemm<BN, true, true, EPI_F32>(m, p, num_sms, s);                   \
     case EPI_F32_ADD: return launch_gemm<BN, true, true, EPI_F32_ADD>(m, p, num_sms, s);           \

@@ -235,6 +235,18 @@ class PipelineRunner:
         dist.broadcast(t, src=dist.get_world_size() - 1)
         return [t.reshape(())]
 
+    def evaluate(self, feeds):
+        """Forward-only loss triple (runtime/executor.py Executor.evaluate), summed over the micro-batches on the last stage
+        and shared with every rank."""
+        from ..runtime.executor import Executor
+        from ..runtime.pipeline import run_pipeline_eval
+        Executor._loss_node(self.worker.full)     # the refusals of Executor.evaluate, on the whole plan (every rank raises)
+        acc = run_pipeline_eval(self.worker, self.tasks, feeds)
+        t = acc.reshape(3).to(torch.float64) if acc is not None else torch.zeros(3, dtype=torch.float64, device=self.device)
+        import torch.distributed as dist
+        dist.broadcast(t, src=dist.get_world_size() - 1)
+        return t
+
 
 def build_pipeline(graph: Graph, trainer, stages: int, micro: int, comm_mode: str, seed: int, use_cuda_graph: bool = False):
     from ..runtime.pipeline import StageWorker

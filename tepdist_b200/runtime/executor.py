@@ -356,6 +356,12 @@ class Executor:
         self._graph: Optional[torch.cuda.CUDAGraph] = None
         self._static_in: Dict[str, torch.Tensor] = {}
         self._static_out: List[torch.Tensor] = []
+        # evaluation step (Executor.evaluate): its own node subset, liveness table, static inputs and captured graph
+        self._eval = False
+        self._eval_plan: Optional[Tuple[List[Node], Dict[int, List[Tuple[int, int]]]]] = None
+        self._eval_graph: Optional[torch.cuda.CUDAGraph] = None
+        self._eval_static_in: Dict[str, torch.Tensor] = {}
+        self._eval_static_out: Optional[torch.Tensor] = None
         from .optimizers import HYPER_SIZE    # (the CUDA kernels read the first four entries)
         self.hyper = torch.zeros(HYPER_SIZE, dtype=torch.float32, device=self.device)
         self._hyper_host = (torch.zeros(HYPER_SIZE, dtype=torch.float32).pin_memory() if self.device.type == "cuda"
@@ -755,6 +761,124 @@ class Executor:
         self._graph.replay()
         ops._count(self._launches_per_step)
         return self._static_out
+
+    # ------------------------------------------------------------------ evaluation
+    def evaluate(self, feeds: Dict[str, torch.Tensor]) -> torch.Tensor:
+        """Forward-only loss of one batch with dropout off: fp64 [3] = (sum of the token losses, number of tokens whose label is
+        in [0, vocab), number of labels >= vocab), summed over every rank that holds a part of the batch, so every rank gets
+        the same triple.  Labels < 0 are ignored.  Runs the nodes the loss depends on, on this plan's sharded graph and
+        variables; it changes nothing a training step reads (no gradients, optimizer, step counter, dropout counter or
+        learning-rate schedule).  Under use_cuda_graph the second call captures its own graph."""
+        if self._eval_plan is None:
+            self._eval_plan = self._plan_eval(self.g)
+        if not self.use_cuda_graph:
+            return self._run_eval(feeds)
+        if self._eval_graph is None:
+            if not self._eval_static_in:
+                for k, t in feeds.items():
+                    self._eval_static_in[k] = t.to(self.device).clone()
+                s = torch.cuda.Stream()
+                s.wait_stream(torch.cuda.current_stream())
+                with torch.cuda.stream(s):
+                    out = self._run_eval(self._eval_static_in)
+                torch.cuda.current_stream().wait_stream(s)
+                torch.cuda.synchronize()
+                return out
+            for k, t in feeds.items():
+                self._eval_static_in[k].copy_(t, non_blocking=True)
+            torch.cuda.synchronize()
+            self._eval_graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self._eval_graph):
+                self._eval_static_out = self._run_eval(self._eval_static_in)
+            self._eval_launches = self._last_eval_launches
+        else:
+            for k, t in feeds.items():
+                self._eval_static_in[k].copy_(t, non_blocking=True)
+        self._eval_graph.replay()
+        ops._count(self._eval_launches)
+        return self._eval_static_out
+
+    @staticmethod
+    def _loss_node(g: Graph) -> Node:
+        """The graph's softmax_xent loss node; graphs an evaluation step cannot run are refused here."""
+        if any(n.op == "batchnorm" for n in g.nodes):
+            raise ValueError("evaluate: the graph has BatchNorm, which evaluates with running statistics this executor does not keep")
+        xent = [n for n in g.nodes if n.op == "softmax_xent"]
+        if len(xent) != 1:
+            raise ValueError(f"evaluate: the loss must be one softmax_xent node; the graph has {len(xent)}")
+        return xent[0]
+
+    def _plan_eval(self, g: Graph, nodes: Optional[List[Node]] = None) -> Tuple[List[Node], Dict[int, List[Tuple[int, int]]]]:
+        """(nodes, free_after): the nodes the loss depends on, in graph order (`nodes`: a pipeline stage's forward body
+        instead), and after which node each value dies among them."""
+        if nodes is None:
+            need = {self._loss_node(g).id}
+            for n in reversed(g.nodes):
+                if n.id in need:
+                    need |= {v.node for v in n.inputs}
+                    if n.id in self.alias_of:
+                        need.add(self.alias_of[n.id][0])
+            nodes = [n for n in g.nodes if n.id in need]
+        last_use: Dict[Tuple[int, int], int] = {}
+        for n in nodes:
+            for v in n.inputs:
+                last_use[v.key()] = n.id
+            if n.id in self.alias_of:
+                last_use[self.alias_of[n.id]] = n.id
+        free_after: Dict[int, List[Tuple[int, int]]] = {}
+        for k, nid in last_use.items():
+            free_after.setdefault(nid, []).append(k)
+        return nodes, free_after
+
+    def _run_eval(self, feeds: Dict[str, torch.Tensor]) -> torch.Tensor:
+        launches0 = ops.launch_count()
+        nodes, free_after = self._eval_plan
+        out = self.run_eval_nodes(nodes, free_after, {}, feeds, "eval")
+        self._last_eval_launches = ops.launch_count() - launches0
+        return out
+
+    def run_eval_nodes(self, nodes: List[Node], free_after: Dict[int, List[Tuple[int, int]]],
+                       env: Dict[Tuple[int, int], torch.Tensor], feeds: Dict[str, torch.Tensor], tag: Any) -> Optional[torch.Tensor]:
+        """Run `nodes` in evaluation mode; returns the loss triple of the softmax_xent node among them (None if there is
+        none).  The side tables the forward kernels fill under `tag` are emptied again, so no training step sees them."""
+        triple = None
+        self._eval, tag0 = True, self._tag
+        self._tag = tag
+        try:
+            for n in nodes:
+                if n.op in ("boundary", "state"):
+                    continue
+                if n.id in self.alias_of:
+                    outs = [env[self.alias_of[n.id]]]
+                else:
+                    self._env = env
+                    outs = self._exec(n, [env[v.key()] for v in n.inputs], feeds)
+                if n.op == "softmax_xent":
+                    triple = self._eval_reduce(n, outs[0])
+                for i, t in enumerate(outs):
+                    env[(n.id, i)] = t
+                for k in free_after.get(n.id, ()):
+                    env.pop(k, None)
+        finally:
+            self._eval, self._tag = False, tag0
+            self._env = None
+            for table in (self.ln_stats, self.bn_stats, self.bn_sync_stats, self._moe_routes):
+                for k in [k for k in table if k[0] == tag]:
+                    del table[k]
+        return triple
+
+    def _eval_reduce(self, n: Node, triple: torch.Tensor) -> torch.Tensor:
+        """Sum the local (loss, tokens, bad labels) triple over the mesh levels that split the loss's tokens (recorded by
+        the SPMD transform as token_levels); levels that replicate the loss, and a pipeline's micro-batch level, are not
+        summed."""
+        if self.collective is None or self.collective.mesh.world == 1 or self.collective.dry:
+            return triple
+        import torch.distributed as dist
+        for lvl, num in zip(n.attrs.get("token_levels", []), n.attrs.get("token_nums", [])):
+            pg = self.collective.mesh.group(int(lvl))
+            if int(num) > 1 and pg is not None:
+                dist.all_reduce(triple, group=pg)
+        return triple
 
     def _set_hyper(self) -> None:
         if self.has_dropout:
@@ -1427,6 +1551,9 @@ class Executor:
             if a.get("residual"):
                 res = ins[k]
             x2 = x.reshape(-1, x.shape[-1])
+            if n.id in self.gelu_dual and self._eval:     # the pre-activation is only kept for backward
+                act = ops.gemm(x2, w, bias=bias, act="gelu", out_dtype=x.dtype).view(*x.shape[:-1], w.shape[0])
+                return [act, act]
             if n.id in self.gelu_dual:
                 pre = torch.empty(x2.shape[0], w.shape[0], dtype=x.dtype, device=dev)
                 act = torch.empty_like(pre)
@@ -1461,6 +1588,11 @@ class Executor:
             out = self._grad_out(n, 0, n.outputs[0].shape)
             ops.colsum_acc(ins[0], out)
             return [out]
+        if op in DROPOUT_OPS and self._eval:     # dropout off: identity, dropout_add a plain add
+            if op != "dropout_add":
+                return [ins[0]]
+            y = ops.ew_native("add", ins[0], ins[1]) if ins[0].is_cuda else None
+            return [y if y is not None else ins[0] + ins[1]]
         if op in DROPOUT_OPS:
             return [ops.dropout(ins[0], a["p"], self._drop_rng(n), ins[1] if op == "dropout_add" else None)]
         if op == "gelu":
@@ -1474,7 +1606,7 @@ class Executor:
             D = C3 // 3 // H
             q5 = qkv.view(B, S, H, 3, D)  # heads-major: a last-dim split is a split over heads
             ds = ins[1] if len(ins) > 1 else None
-            pdrop = float(a.get("pdrop", 0.0))
+            pdrop = 0.0 if self._eval else float(a.get("pdrop", 0.0))
             ring = self._ring(n)
             if ring is not None:    # context parallel: S is this rank's block of the sequence, K / V blocks ride the ring
                 if ds is not None:
@@ -1512,6 +1644,8 @@ class Executor:
             logits, labels = ins
             Vp = logits.shape[-1]
             l2 = logits.reshape(-1, Vp)
+            if self._eval:     # -> the (loss sum, valid tokens, bad labels) triple of this shard; no dlogits
+                return [ops.xent_fwd(l2, labels.reshape(-1), a.get("vocab", Vp))[0]]
             T = int(a.get("global_tokens", l2.shape[0]))  # batch-sharded: partial sum of the GLOBAL mean
             total, _rows = ops.xent_fwd_bwd(l2, labels.reshape(-1), a.get("vocab", Vp), 1.0 / T)
             return [total.reshape(()), l2.view(logits.shape)]

@@ -445,6 +445,66 @@ class StageWorker:
 
     _threaded: Dict[int, Dict[Tuple[int, int], torch.Tensor]] = {}
 
+    def evaluate_forward(self, m: int, feeds: Dict[str, torch.Tensor]) -> None:
+        """Micro-batch m's forward body, eagerly and in evaluation mode (Executor.run_eval_nodes); on the stage that holds
+        the loss its triple is added into eval_acc."""
+        ex = self.exec
+        if self._eval_free is None:
+            # nodes downstream of the loss (the reduction of the loss output a plan may add) have no use in an evaluation
+            after = {n.id for n in self.fwd_nodes if n.op == "softmax_xent"}
+            for n in self.fwd_nodes:
+                if any(v.node in after for v in n.inputs):
+                    after.add(n.id)
+            self._eval_nodes = [n for n in self.fwd_nodes if n.op == "softmax_xent" or n.id not in after]
+            self._eval_free = ex._plan_eval(self.sub, self._eval_nodes)[1]
+            out = self._values_for(self.stage, False) if self.stage < self.S - 1 else []
+            sent = {(self.idmap[k[0]], k[1]) if k[0] in self.idmap else (self.boundary_in.get(k), 0) for k in out}
+            for ks in self._eval_free.values():     # values sent to the next stage live until the Send task
+                ks[:] = [k for k in ks if k not in sent]
+        ex.coords[self.micro_level] = m
+        t = ex.run_eval_nodes(self._eval_nodes, self._eval_free, self._micro_env(m), feeds, ("eval", m))
+        if t is not None:
+            self.eval_acc = t.clone() if self.eval_acc is None else self.eval_acc + t
+
+    eval_acc: Optional[torch.Tensor] = None
+    _eval_free: Optional[Dict[int, List[Tuple[int, int]]]] = None
+    _eval_nodes: List[Node] = []
+
+
+def run_pipeline_eval(worker: StageWorker, task_list: List[Dict[str, Any]], feeds: Dict[str, torch.Tensor]) -> Optional[torch.Tensor]:
+    """One evaluation pass: this device's task list without the backward tasks and the optimizer (AG); every stage body runs
+    eagerly with dropout off.  Returns the loss triple summed over the micro-batches on the stage that holds the loss, None
+    elsewhere.  Nothing of the training step's state is touched: receive buffers are fresh (not the slot ring the captured
+    bodies read), and every micro-batch environment is released by the end of the call."""
+    worker.eval_acc = None
+    worker.env.clear()
+    worker._threaded = {}
+    use_graph, worker.use_graph = worker.use_graph, False     # (recv: fresh buffers instead of the graph slots' ring)
+    pending_recv: Dict[int, List[Any]] = {}
+    pending_send: List[Any] = []
+    try:
+        for t in task_list:
+            kind, m, bwd = t["type"], t["micro"], t["backward"]
+            if not bwd:
+                if kind == "Recv":
+                    pending_recv[m] = worker.recv(m, False, -1)
+                elif kind == "Input":
+                    for w in pending_recv.pop(m, []):
+                        w.wait()
+                elif kind == "Compute":
+                    worker.evaluate_forward(m, feeds)
+                elif kind == "Send":
+                    pending_send += worker.send(m, False)
+            for dead in t.get("release", ()):
+                worker.release(dead)
+        for w, _ in pending_send:
+            w.wait()
+    finally:
+        worker.use_graph = use_graph
+        worker.env.clear()
+        worker._threaded = {}
+    return worker.eval_acc
+
 
 def run_pipeline_step(worker: StageWorker, task_list: List[Dict[str, Any]], feeds: Dict[str, torch.Tensor]) -> Optional[float]:
     """Execute one training step by walking this device's ordered task list."""
